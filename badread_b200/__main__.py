@@ -34,7 +34,7 @@ def main(output=sys.stderr):
 
 def parse_args(args):
     parser = argparse.ArgumentParser(prog='badread', description='Badread: a long read simulator that can imitate '
-                                     'many types of read problems (B200 build of the simulate command)')
+                                     'many types of read problems (GPU build of the simulate command)')
     subparsers = parser.add_subparsers(title='Commands', dest='subparser_name')
     simulate_subparser(subparsers)
     model_subparser(subparsers, 'error_model', 'Build a Badread error model', 7)
@@ -114,7 +114,7 @@ def simulate_subparser(subparsers):
     problem_args.add_argument('--small_plasmid_bias', action='store_true',
                               help='If set, then small circular plasmids are lost when the fragment length is '
                                    'too high (default: small plasmids are included regardless of fragment length)')
-    b200_args = group.add_argument_group('B200')
+    b200_args = group.add_argument_group('GPU')
     b200_args.add_argument('--gpus', type=int, default=1, help='GPUs to shard reads over (default: %(default)s)')
     b200_args.add_argument('--batch_reads', type=int, default=16384,
                            help='Reads per GPU per batch (default: %(default)s)')

@@ -1,4 +1,4 @@
-// bb_kernels.cuh — the per-read hot path as sm_100a kernels.
+// bb_kernels.cuh — the per-read hot path as sm_90a kernels.
 //
 //   K1 bb_k_build_fragments   gather fragments from the HBM-resident reference / literal pool, draw the 2k pad
 //                             bases (simulate.py:260), reset slot states

@@ -34,8 +34,8 @@ struct BBWinTask { int r, a; };  // read, alignment ordinal (1-based: after 25*a
 // something, in order.  The evaluation runs ONE STEP AHEAD of the commit: what an iteration would change depends on its
 // own random stream and on the fragment only, never on earlier commits, and the next step starts at n0 + 128 unless the
 // loop stops - so while warp 0 commits the candidates of step i, warps 1-4 already evaluate step i + 1 into the other
-// half of a double buffer.  A step costs max(evaluate, commit) instead of their sum (the evaluate-then-commit build of
-// round 1 spent 59 % of its warp stall cycles at the CTA barrier between the two: ncu r2s; step 151.4 -> 148.4 ms).  If
+// half of a double buffer.  A step costs max(evaluate, commit) instead of their sum (the evaluate-then-commit build
+// spent most of its warp stall cycles at the CTA barrier between the two).  If
 // the loop stops, the speculative step is simply dropped - the resume point is the commit's.
 #define BB_MUTP_THREADS (BB_WARPS_PER_CTA * 32 + 32)
 
@@ -354,8 +354,8 @@ __device__ __forceinline__ void bb_window_of(int frag_len, unsigned long long se
 // checkpoint: 2 LW + 2 words); the traceback walks the tiles from the last to the first, re-running each tile's columns
 // from its checkpoint into SHARED memory (per-column vertical / horizontal delta words, the two bits per cell edlib's
 // traceback rule needs) and following the path through it.  Round 1 wrote 8 LW bytes per column per window to global
-// memory and read them back along the path - 54 GB per step, with the traceback stalled on those loads 4/5 of the time
-// (ncu: 78 % of the stall cycles on the L1TEX scoreboard, issue slots 18 % busy); now a window moves ~9 KB.
+// memory and read them back along the path, with the traceback stalled on those loads most of the time; now a window
+// moves ~9 KB.
 #define BB_WIN_TILE 16
 #define BB_WIN_CKPT_WORDS(LW) (2 * (LW) + 2)
 #define BB_WIN_MAX_TILES (BB_WIN_MAX_COLS / BB_WIN_TILE)
@@ -505,7 +505,7 @@ bb_k_window_lane(BBBatchDev B, BBErrorModelDev em, const BBWinTask *tasks, const
 // per-column history (Pv, PhRaw per window word) in global memory.  The traceback does not chase it there: the columns
 // ahead of the path are staged in shared memory by cp.async, T columns per tick (bb_ring_tick), so a move costs a
 // shared-memory load instead of an L2 / HBM round trip.  The checkpoint build above (BADREAD_B200_LOWMEM=1) moves ~9 KB
-// per window instead of ~64 KB and measured 14 % slower per step (DESIGN.md section 6).
+// per window instead of ~64 KB and is slower per step: recomputing tiles costs more than the traffic it saves.
 #ifndef BB_WIN_RING_T
 #define BB_WIN_RING_T 4
 #endif

@@ -342,7 +342,7 @@ bb_k_node_lane(BBBatchDev B, BBQueues Q, int parity_order, int *cursor) {
 // ---------------------------------------------------------------------------------------------- lane leaf kernel
 // One leaf per thread, 32 at a time per warp in lock step: forward pass with a checkpoint of the vertical deltas every
 // BB_LEAF_TILE columns, then the traceback tile by tile out of shared memory (the scheme of bb_k_window_lane; round 1
-// kept 64 bytes of history per column per leaf in global memory: 34 GB per step).
+// kept 64 bytes of history per column per leaf in global memory).
 #define BB_LEAF_TILE 16
 #define BB_LEAF_CKPT_WORDS (2 * BB_LEAF_LW + 2)
 #define BB_LEAF_MAX_TILES (BB_LEAF_LANE_COLS / BB_LEAF_TILE)

@@ -55,6 +55,10 @@ int count_common(bool qscores, int device, int k, int max_del, int32_t n_aln, co
         return BB_ERR_ARG;
     }
     BBM_TRY(cudaSetDevice(device));
+    // cudaGetLastError() after the launch below must report this call's launch only: clear whatever an earlier call of
+    // this thread left, e.g. an out-of-memory from an engine's scratch allocation when a second context on the same
+    // GPU did not fit (the engine reported it already)
+    (void)cudaGetLastError();
     const int64_t n_read = read_off[n_aln], n_ref = ref_off[n_aln], n_ops = ops_off[n_aln];
     const int per_slot = qscores ? BBM_NQ : 1;
     DevMem mem;

@@ -1,5 +1,5 @@
 """
-simulate - driver of `badread simulate` on B200, mirroring /root/reference/badread/simulate.py.
+simulate - driver of `badread simulate` on the GPU, mirroring the reference's badread/simulate.py.
 
 What runs where:
   * sequence_fragment (simulate.py:256-358) - the hot path - runs on the GPU for batches of reads

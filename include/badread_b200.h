@@ -1,6 +1,6 @@
 /*
  * badread_b200.h — C ABI of libbadread_b200.so: the drop-in boundary for Badread's per-read
- * error-injection hot path on NVIDIA B200 (sm_100a).
+ * error-injection hot path on NVIDIA H100 (sm_90a).
  *
  * The reference (rrwick/Badread v0.4.2) is pure Python; its only native call on this path is
  * `edlib.align` (third-party).  This ABI is what a ctypes binding inside the reference would bind to replace
@@ -73,7 +73,7 @@ typedef struct bb_read_result {
 /* ---- lifecycle -------------------------------------------------------------------------------------- */
 /* Creates a context on CUDA device `device`. seed is `--seed` (simulate.py:34-36). Fails with BB_ERR_CUDA when
  * there is no usable GPU: there is no CPU path.
- * A context holds BADREAD_B200_SUBBATCHES (environment, default 4, 1..8) workers on the device: large batches are
+ * A context holds BADREAD_B200_SUBBATCHES (environment, default 2, 1..8) workers on the device: large batches are
  * dealt out over them and their kernel chains overlap on separate streams.  Results do not depend on it. */
 BB_API int bb_create(bb_ctx **ctx, int device, uint64_t seed);
 BB_API int bb_destroy(bb_ctx *ctx);

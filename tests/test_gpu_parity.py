@@ -76,6 +76,23 @@ def test_sequence_batch_matches_oracle(engine, error_name, qscore_name):
 def test_large_batch_split_over_workers_matches_oracle(engine):
     """A batch big enough to be dealt out over the context's sub-batch workers (>= 64 reads per worker): every read,
     wherever it ran and wherever its block landed in the output buffers, equals the oracle's."""
+    _check_large_split_batch(engine)
+
+
+def test_head_batch_matches_oracle(monkeypatch):
+    """The same batch on a context of three workers: worker 0 then carries a head batch of the 43 longest reads (3 or
+    more workers and at least 16 reads of >= 0.6x the longest), run by bb_k_mutate_chain on high-priority streams."""
+    from badread_b200.engine import Engine
+    monkeypatch.setenv('BADREAD_B200_SUBBATCHES', '3')
+    monkeypatch.setenv('BADREAD_B200_HEAD_WORKER', '1')
+    eng = Engine(device=0, seed=1234)
+    try:
+        _check_large_split_batch(eng)
+    finally:
+        eng.close()
+
+
+def _check_large_split_batch(engine):
     from badread_b200.engine import FragmentBatch
     em, qm = load_models('nanopore2023', 'nanopore2023')
     O, orc = _oracle(em, qm)

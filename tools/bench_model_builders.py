@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """
 bench_model_builders.py - `badread error_model` / `badread qscore_model` (SURVEY.md 8f row f4) on a synthetic data set,
-this repo's GPU builders next to the unmodified reference (baseline/_ref + oracle/edlib_shim, one process - the
+this repo's GPU builders next to the unmodified reference (oracle/_ref + oracle/edlib_shim, one process - the
 reference's builders are single-threaded Python), with the two model files compared byte for byte.
 
     python tools/bench_model_builders.py [--reads 600] [--length 8000] [--skip_reference]
@@ -126,13 +126,13 @@ def main():
                                 'count on the GPU (bb_count_*: copies + kernels), sort and print'}}
         if not a.skip_reference:
             sys.path.insert(0, os.path.join(ROOT, 'oracle', 'edlib_shim'))
-            sys.path.insert(0, os.path.join(ROOT, 'baseline', '_ref'))
+            sys.path.insert(0, os.path.join(ROOT, 'oracle', '_ref'))
             import badread.error_model as rem
             import badread.qscore_model as rqm
             ref_em, r_em = run(rem.make_error_model, em_args)
             ref_qm, r_qm = run(rqm.make_qscore_model, qm_args)
             res['reference'] = {'error_model': columns / r_em, 'qscore_model': columns / r_qm, 'error_model_s': r_em,
-                                'qscore_model_s': r_qm, 'note': 'unmodified badread (baseline/_ref), one process'}
+                                'qscore_model_s': r_qm, 'note': 'unmodified badread (oracle/_ref), one process'}
             res['parity'] = {'error_model_identical': ours_em == ref_em, 'qscore_model_identical': ours_qm == ref_qm,
                              'error_model_lines': len(ours_em.splitlines()), 'qscore_model_lines': len(ours_qm.splitlines())}
             res['speedup'] = {'error_model': r_em / t_em, 'qscore_model': r_qm / t_qm}

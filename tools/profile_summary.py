@@ -1,7 +1,8 @@
 #!/usr/bin/env python3
 """Aggregates an ncu --csv launch list (tools/profile_step.sh) into profiles/<tag>_{launches.csv,traffic.json,inst.json}.
 The run profiled is `bench.py --profile --steps 1 --warmup 1`: the launches of the SECOND step (the timed one) are kept.
-  profile_summary.py RAW.csv TAG OUTDIR        write the summaries (to OUTDIR and, for the small files, profiles/)
+  profile_summary.py RAW.csv TAG OUTDIR        write the summaries to OUTDIR (copy them into profiles/ and commit them
+                                               to make them the evidence bench.py's roofline object cites)
   profile_summary.py --count RAW.csv KERNEL    launches of KERNEL in the warm-up step (= ncu -s for the timed step)
 """
 import collections
@@ -115,7 +116,7 @@ def main():
     inst = {'source': src, 'warp_inst_G_per_step': round(sum(k['warp_inst_G'] for k in per.values()), 3),
             'thread_inst_G_per_step': round(sum(k['thread_inst_G'] for k in per.values()), 3),
             'per_kernel': {n: k['warp_inst_G'] for n, k in per.items()}}
-    for d in (outdir, 'profiles'):
+    for d in (outdir,):
         os.makedirs(d, exist_ok=True)
         json.dump(traffic, open(os.path.join(d, f'{tag}_traffic.json'), 'w'), indent=1)
         json.dump(inst, open(os.path.join(d, f'{tag}_inst.json'), 'w'), indent=1)
