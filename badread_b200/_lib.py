@@ -85,6 +85,7 @@ def lib():
         'bb_upload_reference': (c.c_int, [vp, vp, i64]),
         'bb_upload_error_model': (c.c_int, [vp, c.c_int, c.c_int, vp, i64, i32, vp, vp, vp, vp, vp, i64]),
         'bb_upload_qscore_model': (c.c_int, [vp, c.c_int, i32, vp, vp, vp, vp]),
+        'bb_upload_qscore_model_cigars': (c.c_int, [vp, c.c_int, i32, vp, vp, vp, vp, vp]),
         'bb_sequence_batch': (c.c_int, [vp, i32, vp, vp, vp, vp, i64, vp, vp, vp, vp, i64, P(i64)]),
         'bb_fetch_last_batch': (c.c_int, [vp, vp, vp, vp, i64, P(i64)]),
         'bb_batch_upload': (c.c_int, [vp, i32, vp, vp, vp, vp, i64, vp]),
@@ -128,7 +129,7 @@ def lib():
 
 
 EXPORTED_SYMBOLS = ['bb_create', 'bb_destroy', 'bb_last_error', 'bb_version', 'bb_upload_reference',
-                    'bb_upload_error_model', 'bb_upload_qscore_model', 'bb_sequence_batch',
+                    'bb_upload_error_model', 'bb_upload_qscore_model', 'bb_upload_qscore_model_cigars', 'bb_sequence_batch',
                     'bb_fetch_last_batch', 'bb_batch_upload', 'bb_batch_run', 'bb_synchronize', 'bb_host_alloc', 'bb_host_free',
                     'bb_last_run_ms', 'bb_stage_name', 'bb_launch_count', 'bb_trace_dump', 'bb_get_qscores', 'bb_align_path',
                     'bb_host_align_kmers', 'bb_host_align_path', 'bb_nccl_available', 'bb_comm_unique_id', 'bb_comm_init_rank',

@@ -57,7 +57,7 @@ struct bb_ctx {
     DevBuf ref; int64_t ref_len = 0;
     bool have_em = false, have_qm = false;
     BBErrorModelDev em{}; DevBuf em_k2r, em_rowoff, em_cum, em_flags, em_slots, em_pool, em_rowinfo;
-    BBQScoreModelDev qm{}; DevBuf qm_hkeys, qm_hvals, qm_rowoff, qm_scores, qm_cum;
+    BBQScoreModelDev qm{}; DevBuf qm_hkeys, qm_hvals, qm_lkeys, qm_lpool, qm_rowoff, qm_scores, qm_cum;
 
     // batch
     int n_reads = 0;
@@ -288,7 +288,7 @@ extern "C" int bb_destroy(bb_ctx *ctx) {
     if (ctx->ev_t0) cudaEventDestroy(ctx->ev_t0);
     if (ctx->ev_t1) cudaEventDestroy(ctx->ev_t1);
     DevBuf *bufs[] = {&ctx->ref, &ctx->em_k2r, &ctx->em_rowoff, &ctx->em_cum, &ctx->em_flags, &ctx->em_slots,
-                      &ctx->em_pool, &ctx->em_rowinfo, &ctx->qm_hkeys, &ctx->qm_hvals, &ctx->qm_rowoff, &ctx->qm_scores, &ctx->qm_cum,
+                      &ctx->em_pool, &ctx->em_rowinfo, &ctx->qm_hkeys, &ctx->qm_hvals, &ctx->qm_lkeys, &ctx->qm_lpool, &ctx->qm_rowoff, &ctx->qm_scores, &ctx->qm_cum,
                       &ctx->d_read_index, &ctx->d_seg_off, &ctx->d_segs, &ctx->d_lit, &ctx->d_target, &ctx->d_order,
                       &ctx->d_reads, &ctx->d_kidx, &ctx->d_frag, &ctx->d_state, &ctx->d_seq, &ctx->d_ops, &ctx->d_dcnt,
                       &ctx->d_qual, &ctx->d_out_seq, &ctx->d_out_qual, &ctx->d_counter, &ctx->s_hist, &ctx->s_hbuf,
@@ -380,38 +380,45 @@ extern "C" int bb_upload_error_model(bb_ctx *ctx, int k, int type, const int32_t
     return BB_OK;
 }
 
-extern "C" int bb_upload_qscore_model(bb_ctx *ctx, int kmer_size, int32_t n_keys, const uint64_t *keys,
-                                      const int32_t *row_off, const uint8_t *scores, const double *cum) {
+extern "C" int bb_upload_qscore_model_cigars(bb_ctx *ctx, int kmer_size, int32_t n_keys, const uint8_t *key_chars,
+                                             const int32_t *key_off, const int32_t *row_off, const uint8_t *scores,
+                                             const double *cum) {
     if (!ctx) return BB_ERR_ARG;
-    if (kmer_size < 1 || (kmer_size & 1) == 0 || n_keys <= 0 || !keys || !row_off || !scores || !cum)
+    if (kmer_size < 1 || (kmer_size & 1) == 0 || n_keys <= 0 || !key_chars || !key_off || !row_off || !scores || !cum)
         return set_err(ctx, BB_ERR_ARG, "qscore model: bad arguments");
     BB_CUDA(ctx, cudaSetDevice(ctx->device));
-    uint32_t bits = 6;
-    while ((1ull << bits) < 2ull * (uint64_t)n_keys) bits++;
-    const size_t hsize = (size_t)1 << bits;
-    std::vector<uint64_t> hk(hsize, 0);
-    std::vector<int32_t> hv(hsize, -1);
-    for (int32_t i = 0; i < n_keys; i++) {
-        if (keys[i] < 4) return set_err(ctx, BB_ERR_ARG, "qscore model: invalid packed key");
-        uint32_t h = (uint32_t)((keys[i] * 0x9E3779B97F4A7C15ull) >> (64 - bits));
-        while (hk[h] != 0 && hk[h] != keys[i]) h = (h + 1) & (uint32_t)(hsize - 1);
-        hk[h] = keys[i]; hv[h] = i;  // a repeated key keeps its last row, like the dict assignment in load_from_file
-    }
+    BBQScoreTables t;
+    std::string err;
+    if (!bb_build_qscore_tables(n_keys, key_chars, key_off, t, err)) return set_err(ctx, BB_ERR_ARG, err);
     const int64_t ne = row_off[n_keys];
     int rc;
-    if ((rc = upload(ctx, ctx->qm_hkeys, hk.data(), hsize))) return rc;
-    if ((rc = upload(ctx, ctx->qm_hvals, hv.data(), hsize))) return rc;
+    if ((rc = upload(ctx, ctx->qm_hkeys, t.hkeys.data(), t.hkeys.size()))) return rc;
+    if ((rc = upload(ctx, ctx->qm_hvals, t.hvals.data(), t.hvals.size()))) return rc;
+    if ((rc = upload(ctx, ctx->qm_lkeys, t.lkeys.data(), t.lkeys.size()))) return rc;
+    if ((rc = upload(ctx, ctx->qm_lpool, t.lpool.data(), t.lpool.size()))) return rc;
     if ((rc = upload(ctx, ctx->qm_rowoff, row_off, (size_t)n_keys + 1))) return rc;
     if ((rc = upload(ctx, ctx->qm_scores, scores, (size_t)ne))) return rc;
     if ((rc = upload(ctx, ctx->qm_cum, cum, (size_t)ne))) return rc;
     BB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    ctx->qm.kmer_size = kmer_size; ctx->qm.hbits = bits;
+    ctx->qm.kmer_size = kmer_size; ctx->qm.hbits = t.hbits;
     ctx->qm.hkeys = ctx->qm_hkeys.as<uint64_t>(); ctx->qm.hvals = ctx->qm_hvals.as<int32_t>();
     ctx->qm.row_off = ctx->qm_rowoff.as<int32_t>(); ctx->qm.scores = ctx->qm_scores.as<uint8_t>();
     ctx->qm.cum = ctx->qm_cum.as<double>();
+    ctx->qm.long_max_len = t.long_max_len; ctx->qm.lbits = t.lbits;
+    ctx->qm.lkeys = ctx->qm_lkeys.as<BBQLongKey>(); ctx->qm.lpool = ctx->qm_lpool.as<uint64_t>();
     ctx->have_qm = true;
     for (bb_ctx *kid : ctx->kids) { kid->qm = ctx->qm; kid->have_qm = true; }  // shared tables
     return BB_OK;
+}
+
+extern "C" int bb_upload_qscore_model(bb_ctx *ctx, int kmer_size, int32_t n_keys, const uint64_t *keys,
+                                      const int32_t *row_off, const uint8_t *scores, const double *cum) {
+    if (!ctx) return BB_ERR_ARG;
+    if (n_keys <= 0 || !keys) return set_err(ctx, BB_ERR_ARG, "qscore model: bad arguments");
+    std::vector<uint8_t> chars;
+    std::vector<int32_t> off;
+    if (!bb_unpack_qscore_keys(n_keys, keys, chars, off)) return set_err(ctx, BB_ERR_ARG, "qscore model: invalid packed key");
+    return bb_upload_qscore_model_cigars(ctx, kmer_size, n_keys, chars.data(), off.data(), row_off, scores, cum);
 }
 
 // Scratch shared by the warp-per-read kernels. hist is sized for the largest traceback edlib's 1 MiB rule

@@ -16,6 +16,7 @@
 #include "../../include/badread_b200.h"
 #include "bb_align.cuh"
 #include "bb_lane.cuh"
+#include "bb_qscore_tables.h"
 #include "bb_rng.cuh"
 
 #define BB_SLOT_NONE 0xFFFFFFFFu
@@ -45,7 +46,7 @@ struct BBErrorModelDev {
     const BBRowInfo *rowinfo;
 };
 
-struct BBQScoreModelDev {
+struct BBQScoreModelDev {  // layout: bb_qscore_tables.h
     int kmer_size;
     const uint64_t *hkeys;  // open addressing, 0 = empty
     const int32_t *hvals;
@@ -53,6 +54,11 @@ struct BBQScoreModelDev {
     const int32_t *row_off;
     const uint8_t *scores;
     const double *cum;
+    // keys longer than 31 symbols
+    int long_max_len;             // symbols of the longest one, 0 = none
+    uint32_t lbits;
+    const BBQLongKey *lkeys;      // open addressing, len 0 = empty
+    const uint64_t *lpool;        // their symbols, 32 per word
 };
 
 struct BBReadDev {
@@ -452,7 +458,7 @@ __global__ void __launch_bounds__(256) bb_k_join(BBBatchDev B, BBErrorModelDev e
 // ------------------------------------------------------------------------------------------------ K5
 __device__ __forceinline__ int bb_qm_find(const BBQScoreModelDev &qm, unsigned long long key) {
     const uint32_t mask = (1u << qm.hbits) - 1u;
-    uint32_t h = (uint32_t)((key * 0x9E3779B97F4A7C15ull) >> (64 - qm.hbits));
+    uint32_t h = bb_qm_slot(key, qm.hbits);
     for (;;) {
         const unsigned long long kk = qm.hkeys[h];
         if (kk == key) return qm.hvals[h];
@@ -461,10 +467,48 @@ __device__ __forceinline__ int bb_qm_find(const BBQScoreModelDev &qm, unsigned l
     }
 }
 
+// Row of the window [s, e] (ops[s] D^dcnt[s] ops[s+1] ... ops[e]) among the keys of more than 31 symbols, -1 if it
+// is none of them.  The walk hashes the symbols as it emits them and stops as soon as the window outgrows the longest
+// such key, so a huge dcnt costs one comparison.  A hash hit is confirmed by walking the window again against the
+// pooled symbols.
+__device__ inline int bb_qm_find_long(const BBQScoreModelDev &qm, const uint8_t *ops, const unsigned int *dcnt, int s, int e) {
+    const int bound = qm.long_max_len;
+    unsigned long long h = BB_QM_LONG_HASH_INIT;
+    int len = 0;
+    for (int x = s; x <= e; x++) {
+        if (len >= bound) return -1;
+        h = bb_qm_long_hash(h, ops[x]);
+        len++;
+        if (x < e) {
+            const unsigned int d = dcnt[x];
+            if (d > (unsigned int)(bound - len)) return -1;
+            for (unsigned int c = 0; c < d; c++) h = bb_qm_long_hash(h, 3u);
+            len += (int)d;
+        }
+    }
+    const uint32_t mask = (1u << qm.lbits) - 1u;
+    for (uint32_t slot = bb_qm_slot(h, qm.lbits);; slot = (slot + 1) & mask) {
+        const BBQLongKey k = qm.lkeys[slot];
+        if (k.len == 0) return -1;
+        if (k.len != len || k.hash != h) continue;
+        const uint64_t *w = qm.lpool + k.off;
+        bool same = true;
+        int j = 0;
+        for (int x = s; x <= e && same; x++) {
+            same = ((w[j >> 5] >> (2 * (j & 31))) & 3u) == ops[x];
+            j++;
+            if (x < e)
+                for (unsigned int c = 0; c < dcnt[x] && same; c++, j++) same = ((w[j >> 5] >> (2 * (j & 31))) & 3u) == 3u;
+        }
+        if (same) return k.row;
+    }
+}
+
 // qscore for base i of a read of n bases given per-base ops and deletion counts (qscore_model.py:54-68 and
 // QScoreModel.get_qscore :273-287).  partial_cigar = ops[s] D^dcnt[s] ops[s+1] ... ops[e]; a CIGAR that is
 // not in the model loses its first and last symbol and then its outer D's, which is exactly the window
-// [s+1, e-1] of the same form.
+// [s+1, e-1] of the same form.  A window of up to 31 symbols is packed into one key of the uint64 table; a longer one
+// goes to the side table (bb_qm_find_long) when the model has long keys.
 __device__ __forceinline__ uint8_t bb_qscore_base(const BBQScoreModelDev &qm, const uint8_t *ops, const unsigned int *dcnt,
                                                   int n, int i, unsigned long long seed, unsigned long long read) {
     int mm = (qm.kmer_size - 1) / 2;
@@ -486,6 +530,7 @@ __device__ __forceinline__ uint8_t bb_qscore_base(const BBQScoreModelDev &qm, co
             }
         }
         if (ok && len <= 31) row = bb_qm_find(qm, key);
+        else if (qm.long_max_len > 0) row = bb_qm_find_long(qm, ops, dcnt, s, e);
     }
     if (row < 0) return 0;  // cannot happen: '=', 'X', 'I' are asserted at model load (qscore_model.py:205-207)
     const int e0 = qm.row_off[row], ne = qm.row_off[row + 1] - e0;

@@ -168,9 +168,10 @@ class Engine(object):
 
     def set_qscore_model(self, qscore_model):
         t = qscore_model.to_device_tables()
-        rc = self._lib.bb_upload_qscore_model(self._ctx, t['kmer_size'], t['n_keys'], _ptr(t['keys']),
-                                              _ptr(t['row_off']), _ptr(t['scores']), _ptr(t['cum']))
-        self._check(rc, 'bb_upload_qscore_model')
+        rc = self._lib.bb_upload_qscore_model_cigars(self._ctx, t['kmer_size'], t['n_keys'], _ptr(t['key_chars']),
+                                                     _ptr(t['key_off']), _ptr(t['row_off']), _ptr(t['scores']),
+                                                     _ptr(t['cum']))
+        self._check(rc, 'bb_upload_qscore_model_cigars')
         self.qscore_model = qscore_model
 
     # ---- batch

@@ -1,12 +1,13 @@
 """
 QScoreModel and get_qscores - host side of the qscore model, same plugin surface as
 /root/reference/badread/qscore_model.py:178-287 (`scores`, `probabilities`, `kmer_size`, `type`, `get_qscore`)
-plus `to_device_tables()` for `bb_upload_qscore_model`, and the module-level `get_qscores(seq, frag, model)`
+plus `to_device_tables()` for `bb_upload_qscore_model_cigars`, and the module-level `get_qscores(seq, frag, model)`
 (qscore_model.py:32-75) which runs on the GPU through the C ABI.
 
-Device table layout: every CIGAR key over {=,X,I,D} is packed two bits per symbol ('='=0, 'X'=1, 'I'=2, 'D'=3)
-under a leading 1 bit (so keys of different lengths never collide; at most 31 symbols); row_off / scores / cum per
-key, cum = list(itertools.accumulate(probabilities)) as random.choices builds it (qscore_model.py:283).
+Device table layout: the CIGAR keys over {=,X,I,D}, of any length, as key_chars / key_off; row_off / scores / cum
+per key, cum = list(itertools.accumulate(probabilities)) as random.choices builds it (qscore_model.py:283).  `keys`
+also gives each key of at most 31 symbols packed two bits per symbol ('='=0, 'X'=1, 'I'=2, 'D'=3) under a leading 1
+bit, the form bb_upload_qscore_model takes; a longer key has no packed form and is 0 there.
 
 Derived from Badread (Copyright 2018 Ryan Wick, rrwick@gmail.com, https://github.com/rrwick/Badread), which is free
 software under the GNU General Public License version 3 or later; this file mirrors the named parts of the
@@ -28,7 +29,7 @@ from .misc import get_open_func
 BUILTIN_MODELS = ('nanopore2018', 'nanopore2020', 'nanopore2023', 'pacbio2016', 'pacbio2021')
 MODEL_DIR = pathlib.Path(os.path.dirname(os.path.realpath(__file__))) / 'models'
 _SYMBOL = {'=': 0, 'X': 1, 'I': 2, 'D': 3}
-MAX_KEY_SYMBOLS = 31
+PACKED_KEY_SYMBOLS = 31    # the most a uint64 holds under its leading 1 bit
 
 
 def pack_cigar(cigar):
@@ -136,20 +137,18 @@ class QScoreModel(object):
                             scores=np.asarray(scores, dtype=np.uint8), probs=np.asarray(probs, dtype=np.float64))
 
     def to_device_tables(self):
-        """Flat arrays for bb_upload_qscore_model (packed keys) and the oracle (key strings)."""
+        """Flat arrays for bb_upload_qscore_model_cigars and the oracle (key strings, any length); `keys` holds the
+        packed form of bb_upload_qscore_model, 0 for a key longer than 31 symbols."""
         keys = list(self.scores.keys())
         packed, key_chars, key_off, row_off = [], [], [0], [0]
         scores, cum = [], []
         for cigar in keys:
             if any(c not in _SYMBOL for c in cigar) or len(cigar) == 0:
                 sys.exit(f'Error: qscore model CIGAR {cigar!r} holds symbols other than =XID')
-            if len(cigar) > MAX_KEY_SYMBOLS:
-                sys.exit(f'Error: qscore model CIGARs longer than {MAX_KEY_SYMBOLS} symbols are not supported '
-                         f'by badread_b200 ({cigar})')
             s, p = self.scores[cigar], self.probabilities[cigar]
             if len(s) == 0 or len(s) != len(p) or min(s) < 0 or max(s) > 93:
                 sys.exit(f'Error: qscore model row {cigar} is malformed')
-            packed.append(pack_cigar(cigar))
+            packed.append(pack_cigar(cigar) if len(cigar) <= PACKED_KEY_SYMBOLS else 0)
             key_chars.append(cigar)
             key_off.append(key_off[-1] + len(cigar))
             scores.extend(s)

@@ -95,8 +95,16 @@ BB_API int bb_upload_error_model(bb_ctx *ctx, int k, int type, const int32_t *km
                           const uint8_t *pool, int64_t pool_len);
 
 /* Qscore model tables (flat form of QScoreModel.scores / .probabilities, qscore_model.py:178-271).
- *  keys[n_keys]: CIGAR strings over {=,X,I,D} packed 2 bits per symbol under a leading 1 bit (<= 31 symbols);
- *  row_off[n_keys+1]; scores / cum per entry. kmer_size as QScoreModel.kmer_size. */
+ *  Key i is the CIGAR string key_chars[key_off[i] .. key_off[i+1]) over {=,X,I,D}, of any length;
+ *  row_off[n_keys+1]; scores / cum per entry. kmer_size as QScoreModel.kmer_size.  A repeated key keeps its last row
+ *  (the dict assignment of QScoreModel.load_from_file).  An empty key or a symbol outside =XID is rejected
+ *  (BB_ERR_ARG, message in bb_last_error). */
+BB_API int bb_upload_qscore_model_cigars(bb_ctx *ctx, int kmer_size, int32_t n_keys, const uint8_t *key_chars,
+                                         const int32_t *key_off, const int32_t *row_off, const uint8_t *scores,
+                                         const double *cum);
+
+/* The same tables with keys[n_keys] packed 2 bits per symbol ('='=0, 'X'=1, 'I'=2, 'D'=3) under a leading 1 bit, which
+ *  limits a key to 31 symbols; bb_upload_qscore_model_cigars takes keys of any length. */
 BB_API int bb_upload_qscore_model(bb_ctx *ctx, int kmer_size, int32_t n_keys, const uint64_t *keys, const int32_t *row_off,
                            const uint8_t *scores, const double *cum);
 
