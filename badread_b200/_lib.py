@@ -19,6 +19,8 @@ BB_OK = 0
 BB_ERR_CUDA, BB_ERR_ARG, BB_ERR_STATE, BB_ERR_CAPACITY, BB_ERR_INTERNAL = -1, -2, -3, -4, -5
 BB_SEG_REF_FWD, BB_SEG_REF_REV, BB_SEG_LITERAL = 0, 1, 2
 BB_N_STAGES = 8
+# bb_rerun_reason: what made a batch run again (bb_last_run_retries)
+BB_RERUN_ROUNDS, BB_RERUN_SLACK, BB_RERUN_LEVELS, BB_RERUN_QUEUES, BB_RERUN_SCRATCH = 1, 2, 4, 8, 16
 
 
 class Segment(ctypes.Structure):
@@ -91,6 +93,7 @@ def lib():
         'bb_batch_upload': (c.c_int, [vp, i32, vp, vp, vp, vp, i64, vp]),
         'bb_batch_run': (c.c_int, [vp]),
         'bb_synchronize': (c.c_int, [vp]),
+        'bb_last_run_retries': (c.c_int, [vp, P(i32), P(c.c_uint32)]),
         'bb_host_alloc': (c.c_int, [P(vp), i64]),
         'bb_host_free': (c.c_int, [vp]),
         'bb_last_run_ms': (c.c_int, [vp, P(c.c_float), P(c.c_float)]),
@@ -130,7 +133,8 @@ def lib():
 
 EXPORTED_SYMBOLS = ['bb_create', 'bb_destroy', 'bb_last_error', 'bb_version', 'bb_upload_reference',
                     'bb_upload_error_model', 'bb_upload_qscore_model', 'bb_upload_qscore_model_cigars', 'bb_sequence_batch',
-                    'bb_fetch_last_batch', 'bb_batch_upload', 'bb_batch_run', 'bb_synchronize', 'bb_host_alloc', 'bb_host_free',
+                    'bb_fetch_last_batch', 'bb_batch_upload', 'bb_batch_run', 'bb_synchronize', 'bb_last_run_retries',
+                    'bb_host_alloc', 'bb_host_free',
                     'bb_last_run_ms', 'bb_stage_name', 'bb_launch_count', 'bb_trace_dump', 'bb_get_qscores', 'bb_align_path',
                     'bb_host_align_kmers', 'bb_host_align_path', 'bb_nccl_available', 'bb_comm_unique_id', 'bb_comm_init_rank',
                     'bb_comm_init_all', 'bb_allreduce_bases', 'bb_allreduce_bases_all', 'bb_planner_create', 'bb_planner_destroy',

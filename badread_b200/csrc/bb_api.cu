@@ -37,6 +37,8 @@ struct DevBuf {  // grow-only device allocation
     template <typename T> T *as() const { return reinterpret_cast<T *>(p); }
 };
 
+constexpr int BB_MAX_ROUNDS = 15;  // error-loop rounds a run can enqueue (16 counters each, see BB_ROUND_BASE)
+
 const char *kStageNames[BB_N_STAGES] = {"build_fragments", "error_loop", "scan", "join", "final_align", "qscores",
                                         "compact", "total"};
 
@@ -75,10 +77,13 @@ struct bb_ctx {
     int n_levels = 0;          // Hirschberg levels enqueued (from the longest fragment)
     int extra_levels = 0;
     bool lr_worst = false;     // size the split-score scratch for the worst case instead of the expected edit count
+    int lr_cap = 0;            // > 0: split-score scratch of a batch starts at this many rows (BADREAD_B200_LR_CAP)
     struct RunInfo { BBScanOut scan; int counters[256]; int qcount[2][32]; } *h_info = nullptr;  // pinned
     std::vector<BBReadDev> h_res;  // per-read records of the finished run
     bool finished = false;
     bool reran = false;        // w_finish had to run the batch again (copies enqueued before that are stale)
+    int n_reruns = 0;          // runs of the current batch after the first (bb_last_run_retries)
+    uint32_t rerun_reasons = 0;  // BB_RERUN_* bits of what did not fit
     DevBuf d_scan;
     void *nccl_comm = nullptr;   // ncclComm_t of this context's device (bb_comm_init_rank / bb_comm_init_all)
     DevBuf d_red;                // two int64: send, receive of bb_allreduce_bases
@@ -252,6 +257,11 @@ static int create_worker(bb_ctx **out, int device, uint64_t seed, bool high_prio
     if (const char *e = std::getenv("BADREAD_B200_LOWMEM")) ctx->lowmem = (e[0] != '0');
     if (const char *e = std::getenv("BADREAD_B200_LPT")) ctx->lpt_order = (e[0] != '0');
     if (const char *e = std::getenv("BADREAD_B200_RING_T")) ctx->ring_t = (e[0] == '8') ? 8 : (e[0] == '2') ? 2 : 4;
+    // starting values of the limits w_finish grows when a batch outgrows them (the results do not depend on them)
+    if (const char *e = std::getenv("BADREAD_B200_ROUNDS")) ctx->n_rounds = std::max(1, std::min(BB_MAX_ROUNDS, std::atoi(e)));
+    if (const char *e = std::getenv("BADREAD_B200_SLACK")) { const double v = std::atof(e); if (v > 0.0) ctx->slack = v; }
+    if (const char *e = std::getenv("BADREAD_B200_EXTRA_LEVELS")) ctx->extra_levels = std::atoi(e);
+    if (const char *e = std::getenv("BADREAD_B200_LR_CAP")) ctx->lr_cap = std::max(0, std::atoi(e));
     *out = ctx;
     return BB_OK;
 }
@@ -423,14 +433,14 @@ extern "C" int bb_upload_qscore_model(bb_ctx *ctx, int kmer_size, int32_t n_keys
 
 // Scratch shared by the warp-per-read kernels. hist is sized for the largest traceback edlib's 1 MiB rule
 // admits (ceil(n/64)*m < 52429 -> < 104858 32-row blocks); tbuf holds a joined 1000-slot window.
-static int ensure_scratch(bb_ctx *ctx, int hbuf_need, int lr_need, int len_need) {
+static int ensure_scratch(bb_ctx *ctx, int hbuf_need, int lr_need, int len_need, int lr_floor = 4096) {
     const int n_warps = ctx->n_warps;
     const int hist_cap = 106496;
     const int tbuf_stride = 1000 * 255 + 1024;
     const int stack_cap = 64;
     int hbuf_cap = std::max(hbuf_need + 64, tbuf_stride);
     hbuf_cap = (hbuf_cap + 255) & ~255;
-    int lr_cap = std::max(lr_need + 64, 4096);
+    int lr_cap = std::max(lr_need + 64, lr_floor);
     lr_cap = (lr_cap + 255) & ~255;
     int peq_cap = bb_peq_words(len_need) + 8;
     peq_cap = (peq_cap + 63) & ~63;
@@ -489,7 +499,6 @@ static BBBatchDev batch_dev(bb_ctx *ctx) {
 // Counters of a run live in d_counter (256 ints, cleared once per run): [0, 16) spare; round r of the error loop owns
 // the 16 ints from BB_ROUND_BASE(r).
 #define BB_N_COUNTERS 256
-#define BB_MAX_ROUNDS 15
 #define BB_ROUND_BASE(r) (16 + 16 * (r))
 enum { BBC_MUTATE = 0, BBC_NTASKS = 1, BBC_LANE4 = 2, BBC_FB1 = 3, BBC_LANE8 = 4, BBC_FB2 = 5, BBC_WARP = 6, BBC_PENDING = 7 };
 
@@ -540,16 +549,18 @@ static int w_prepare(bb_ctx *ctx) {
         if (ctx->lowmem) BB_CUDA(ctx, ctx->s_wckpt.ensure(2 * lanes * BB_WIN_MAX_TILES * BB_WIN_CKPT_WORDS(BB_WIN_LW) * sizeof(uint32_t)));
     }
     // per-warp scratch: strip carries / bitmaps for the longest joined read; split-score arrays for the widest band
-    // (expected: a few times the injected edits; worst case: the whole read)
+    // (expected: a few times the injected edits; worst case: the whole read; BADREAD_B200_LR_CAP replaces the expected
+    // size and its floor)
     const int len_b = (int)std::min<double>((double)ctx->max_len * ctx->slack + 64.0, (double)(1 << 24));
-    int lr_need = 4096;
+    const int lr_floor = ctx->lr_cap > 0 ? ctx->lr_cap : 4096;
+    int lr_need = lr_floor;
     for (int r = 0; r < n; r++) {
         const double len = (double)ctx->h_reads[(size_t)r].frag_len;
         const double worst = len * ctx->slack + 64.0;
-        const double expect = 3.0 * (1.0 - ctx->h_target[(size_t)r]) * len + 0.02 * len + 512.0;
+        const double expect = ctx->lr_cap > 0 ? 0.0 : 3.0 * (1.0 - ctx->h_target[(size_t)r]) * len + 0.02 * len + 512.0;
         lr_need = std::max(lr_need, (int)std::min(worst, ctx->lr_worst ? worst : expect));
     }
-    int rc = ensure_scratch(ctx, len_b, lr_need, len_b);
+    int rc = ensure_scratch(ctx, len_b, lr_need, len_b, lr_floor);
     if (rc) return rc;
     const int cap_node = (int)std::min<int64_t>(ctx->seq_cap / 256 + 4ll * n + 1024, 0x7ffffff0);
     for (int s = 0; s < 2; s++) {
@@ -559,7 +570,7 @@ static int w_prepare(bb_ctx *ctx) {
         for (int w = 0; w < 2; w++) BB_CUDA(ctx, qb.leaf[w].ensure((size_t)cap_node * sizeof(BBNode)));
         BB_CUDA(ctx, qb.count.ensure(512 * sizeof(int)));
     }
-    ctx->n_levels = std::min(48, level_bound(ctx->max_len, ctx->slack) + ctx->extra_levels);
+    ctx->n_levels = std::max(1, std::min(48, level_bound(ctx->max_len, ctx->slack) + ctx->extra_levels));
     return BB_OK;
 }
 
@@ -844,14 +855,14 @@ static int w_finish(bb_ctx *ctx) {
         BB_CUDA(ctx, cudaMemcpyAsync(ctx->h_res.data(), ctx->d_reads.p, (size_t)n * sizeof(BBReadDev), cudaMemcpyDeviceToHost, ctx->stream));
         BB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
         const bb_ctx::RunInfo &info = *ctx->h_info;
-        bool again = false;
+        uint32_t again = 0;
         std::string why;
         if (info.counters[BB_ROUND_BASE(ctx->n_rounds - 1) + BBC_PENDING] > 0 || info.scan.n_pending > 0) {
-            ctx->n_rounds = std::min(BB_MAX_ROUNDS, ctx->n_rounds + 3); again = true; why += " error-loop rounds";
+            ctx->n_rounds = std::min(BB_MAX_ROUNDS, ctx->n_rounds + 3); again |= BB_RERUN_ROUNDS; why += " error-loop rounds";
         }
         if (info.scan.n_nospace > 0) {  // (reads still pending after the last round are counted separately)
             const double need = (double)std::max(info.scan.seq_total, info.scan.out_total) / (double)std::max<int64_t>(1, ctx->frag_total);
-            ctx->slack = std::max(ctx->slack * 1.5, need * 1.1 + 0.05); again = true; why += " buffer slack";
+            ctx->slack = std::max(ctx->slack * 1.5, need * 1.1 + 0.05); again |= BB_RERUN_SLACK; why += " buffer slack";
         }
         const int last_parity = ctx->n_levels & 1;  // the queues the level after the last one would read
         int left = 0, overflow = 0;
@@ -859,15 +870,17 @@ static int w_finish(bb_ctx *ctx) {
             for (int c = 0; c < BBQ_NODE_CLASSES; c++) left += info.qcount[s][BBQ_COUNT(c, last_parity)];
             overflow += info.qcount[s][BBQ_OVERFLOW];
         }
-        if (left > 0) { ctx->extra_levels += 8; again = true; why += " levels"; }
-        if (overflow) { ctx->slack *= 1.5; again = true; why += " task queues"; }
+        if (left > 0) { ctx->extra_levels += 8; again |= BB_RERUN_LEVELS; why += " levels"; }
+        if (overflow) { ctx->slack *= 1.5; again |= BB_RERUN_QUEUES; why += " task queues"; }
         for (int r = 0; r < n && !ctx->lr_worst; r++) {
             const int f = (ctx->h_res[(size_t)r].flags & ~BB_FLAG_NOSPACE) >> 8;
-            if (f & (16 | 4 | 2)) { ctx->lr_worst = true; ctx->slack *= 1.25; again = true; why += " alignment scratch"; }
+            if (f & (16 | 4 | 2)) { ctx->lr_worst = true; ctx->slack *= 1.25; again |= BB_RERUN_SCRATCH; why += " alignment scratch"; }
         }
         if (!again) break;
         ctx->reran = true;
+        ctx->rerun_reasons |= again;
         if (attempt >= 3) return set_err(ctx, BB_ERR_INTERNAL, "batch did not fit after growing:" + why);
+        ctx->n_reruns++;
         int rc = w_prepare(ctx);
         if (rc) return rc;
         if ((rc = w_enqueue(ctx))) return rc;
@@ -1033,7 +1046,10 @@ extern "C" int bb_batch_upload(bb_ctx *ctx, int32_t n_reads, const uint64_t *rea
 extern "C" int bb_batch_run(bb_ctx *ctx) {
     if (!ctx) return BB_ERR_ARG;
     const int S = ctx->n_split;
-    for (int w = 0; w < S; w++) worker_of(ctx, w)->reran = false;
+    for (int w = 0; w < S; w++) {
+        bb_ctx *wk = worker_of(ctx, w);
+        wk->reran = false; wk->n_reruns = 0; wk->rerun_reasons = 0;
+    }
     BB_CUDA(ctx, cudaSetDevice(ctx->device));
     BB_CUDA(ctx, cudaEventRecord(ctx->ev_t0, ctx->stream));
     for (int w = 1; w < S; w++) BB_CUDA(ctx, cudaStreamWaitEvent(worker_of(ctx, w)->stream, ctx->ev_t0, 0));
@@ -1043,6 +1059,20 @@ extern "C" int bb_batch_run(bb_ctx *ctx) {
     }
     for (int w = 1; w < S; w++) BB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, worker_of(ctx, w)->ev[BB_N_STAGES - 1], 0));
     BB_CUDA(ctx, cudaEventRecord(ctx->ev_t1, ctx->stream));
+    return BB_OK;
+}
+
+extern "C" int bb_last_run_retries(const bb_ctx *ctx, int32_t *n_reruns, uint32_t *reasons) {
+    if (!ctx) return BB_ERR_ARG;
+    int32_t total = 0;
+    uint32_t bits = 0;
+    for (int w = 0; w < ctx->n_split; w++) {
+        const bb_ctx *wk = w == 0 ? ctx : ctx->kids[(size_t)w - 1];
+        total += wk->n_reruns;
+        bits |= wk->rerun_reasons;
+    }
+    if (n_reruns) *n_reruns = total;
+    if (reasons) *reasons = bits;
     return BB_OK;
 }
 
@@ -1162,7 +1192,8 @@ extern "C" int bb_sequence_batch(bb_ctx *ctx, int32_t n_reads, const uint64_t *r
         BB_CUDA(ctx, cudaEventSynchronize(wk->ev_scan));
         base[(size_t)w] = total;
         total += wk->h_info->scan.out_total;
-        if (wk->h_info->scan.n_nospace > 0 || total > out_cap) { eager = false; break; }
+        // (a worker with reads that did not fit or did not finish runs again: its size and everything after it moves)
+        if (wk->h_info->scan.n_nospace > 0 || wk->h_info->scan.n_pending > 0 || total > out_cap) { eager = false; break; }
         if ((rc = w_copy_out(wk, base[(size_t)w], seq_out, qual_out))) { eager = false; break; }
     }
     return fetch_all(ctx, results, seq_out, qual_out, out_cap, out_total, eager ? &base : nullptr);

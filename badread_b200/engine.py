@@ -217,6 +217,14 @@ class Engine(object):
         names = [self._lib.bb_stage_name(i).decode() for i in range(_lib.BB_N_STAGES)]
         return total.value, dict(zip(names, [float(x) for x in stages]))
 
+    def last_run_retries(self):
+        """(re-runs, reason bits) of the last batch: how often a fetch had to run it again because a limit sized from
+        the fragment lengths was too small, summed over the workers, and the _lib.BB_RERUN_* bits of those limits."""
+        n = ctypes.c_int32(0)
+        reasons = ctypes.c_uint32(0)
+        self._check(self._lib.bb_last_run_retries(self._ctx, ctypes.byref(n), ctypes.byref(reasons)), 'bb_last_run_retries')
+        return int(n.value), int(reasons.value)
+
     def launch_count(self):
         return int(self._lib.bb_launch_count(self._ctx))
 

@@ -135,6 +135,21 @@ BB_API int bb_batch_upload(bb_ctx *ctx, int32_t n_reads, const uint64_t *read_in
                     const double *target_identity);
 BB_API int bb_batch_run(bb_ctx *ctx);
 BB_API int bb_synchronize(bb_ctx *ctx);
+/* A batch run is enqueued with buffers, error-loop rounds, Hirschberg levels and scratch sized from the fragment lengths.
+ * When the device reports that one of them was too small, the fetch raises it and runs the batch again (at most three
+ * times; then it fails with "batch did not fit after growing").  Raised limits stay on the context.  This reports the
+ * re-runs of the last bb_batch_run, summed over the workers, and the BB_RERUN_* bits of what did not fit; complete once
+ * the batch has been fetched.  Environment variables read at bb_create set the starting limits:
+ * BADREAD_B200_ROUNDS (1..15, default 3), BADREAD_B200_SLACK (> 0, default 1.25), BADREAD_B200_EXTRA_LEVELS (default 0,
+ * may be negative), BADREAD_B200_LR_CAP (split-score rows, default: from the expected edits, at least 4096). */
+enum bb_rerun_reason {
+    BB_RERUN_ROUNDS = 1,   /* reads still in the error loop after the last round */
+    BB_RERUN_SLACK = 2,    /* joined reads longer than the read buffers */
+    BB_RERUN_LEVELS = 4,   /* Hirschberg nodes left after the last level */
+    BB_RERUN_QUEUES = 8,   /* node queues overflowed */
+    BB_RERUN_SCRATCH = 16  /* per-warp alignment scratch too small */
+};
+BB_API int bb_last_run_retries(const bb_ctx *ctx, int32_t *n_reruns, uint32_t *reasons);
 /* CUDA-event time (ms) of the last bb_batch_run on the ctx stream, total and per stage
  * (stage_ms[BB_N_STAGES], see bb_stage_name). Synchronizes. */
 #define BB_N_STAGES 8
