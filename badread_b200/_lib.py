@@ -86,6 +86,7 @@ def lib():
         'bb_version': (c.c_char_p, []),
         'bb_upload_reference': (c.c_int, [vp, vp, i64]),
         'bb_upload_error_model': (c.c_int, [vp, c.c_int, c.c_int, vp, i64, i32, vp, vp, vp, vp, vp, i64]),
+        'bb_upload_error_model_kmers': (c.c_int, [vp, c.c_int, i32, vp, vp, vp, vp, vp, vp, i64]),
         'bb_upload_qscore_model': (c.c_int, [vp, c.c_int, i32, vp, vp, vp, vp]),
         'bb_upload_qscore_model_cigars': (c.c_int, [vp, c.c_int, i32, vp, vp, vp, vp, vp]),
         'bb_sequence_batch': (c.c_int, [vp, i32, vp, vp, vp, vp, i64, vp, vp, vp, vp, i64, P(i64)]),
@@ -119,6 +120,8 @@ def lib():
         'bb_fastq_format_sharded': (c.c_int, [i32, vp, vp, vp, vp, i32, i64, i64, i32, vp, i64, P(i64), P(i32), P(i64), P(i32)]),
         'bb_count_kmer_alternatives': (c.c_int, [c.c_int, c.c_int, i32, vp, vp, vp, vp, vp, vp, vp, vp, i64, vp, vp, vp, P(i64),
                                                  i64, vp, vp, vp, P(i64)]),
+        'bb_count_kmer_alternatives_wide': (c.c_int, [c.c_int, c.c_int, i32, vp, vp, vp, vp, vp, vp, vp, vp, i64, vp, vp, vp,
+                                                      P(i64), i64, vp, vp, vp, P(i64)]),
         'bb_count_cigar_qscores': (c.c_int, [c.c_int, c.c_int, c.c_int, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, i64, vp, vp, vp,
                                              P(i64), vp, i64, vp, vp, vp, P(i64)]),
         'bb_model_error': (c.c_char_p, []),
@@ -132,11 +135,11 @@ def lib():
 
 
 EXPORTED_SYMBOLS = ['bb_create', 'bb_destroy', 'bb_last_error', 'bb_version', 'bb_upload_reference',
-                    'bb_upload_error_model', 'bb_upload_qscore_model', 'bb_upload_qscore_model_cigars', 'bb_sequence_batch',
+                    'bb_upload_error_model', 'bb_upload_error_model_kmers', 'bb_upload_qscore_model', 'bb_upload_qscore_model_cigars', 'bb_sequence_batch',
                     'bb_fetch_last_batch', 'bb_batch_upload', 'bb_batch_run', 'bb_synchronize', 'bb_last_run_retries',
                     'bb_host_alloc', 'bb_host_free',
                     'bb_last_run_ms', 'bb_stage_name', 'bb_launch_count', 'bb_trace_dump', 'bb_get_qscores', 'bb_align_path',
                     'bb_host_align_kmers', 'bb_host_align_path', 'bb_nccl_available', 'bb_comm_unique_id', 'bb_comm_init_rank',
                     'bb_comm_init_all', 'bb_allreduce_bases', 'bb_allreduce_bases_all', 'bb_planner_create', 'bb_planner_destroy',
                     'bb_planner_plan', 'bb_planner_view', 'bb_planner_error', 'bb_fastq_format', 'bb_fastq_format_sharded',
-                    'bb_count_kmer_alternatives', 'bb_count_cigar_qscores', 'bb_model_error']
+                    'bb_count_kmer_alternatives', 'bb_count_kmer_alternatives_wide', 'bb_count_cigar_qscores', 'bb_model_error']

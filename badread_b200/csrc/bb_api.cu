@@ -59,6 +59,7 @@ struct bb_ctx {
     DevBuf ref; int64_t ref_len = 0;
     bool have_em = false, have_qm = false;
     BBErrorModelDev em{}; DevBuf em_k2r, em_rowoff, em_cum, em_flags, em_slots, em_pool, em_rowinfo;
+    BBEmHashDev em_hash{}; DevBuf em_hentries;  // k-mer index as a hash table (bb_upload_error_model_kmers)
     BBQScoreModelDev qm{}; DevBuf qm_hkeys, qm_hvals, qm_lkeys, qm_lpool, qm_rowoff, qm_scores, qm_cum;
 
     // batch
@@ -297,7 +298,7 @@ extern "C" int bb_destroy(bb_ctx *ctx) {
     cudaStreamSynchronize(ctx->stream);
     if (ctx->ev_t0) cudaEventDestroy(ctx->ev_t0);
     if (ctx->ev_t1) cudaEventDestroy(ctx->ev_t1);
-    DevBuf *bufs[] = {&ctx->ref, &ctx->em_k2r, &ctx->em_rowoff, &ctx->em_cum, &ctx->em_flags, &ctx->em_slots,
+    DevBuf *bufs[] = {&ctx->ref, &ctx->em_k2r, &ctx->em_hentries, &ctx->em_rowoff, &ctx->em_cum, &ctx->em_flags, &ctx->em_slots,
                       &ctx->em_pool, &ctx->em_rowinfo, &ctx->qm_hkeys, &ctx->qm_hvals, &ctx->qm_lkeys, &ctx->qm_lpool, &ctx->qm_rowoff, &ctx->qm_scores, &ctx->qm_cum,
                       &ctx->d_read_index, &ctx->d_seg_off, &ctx->d_segs, &ctx->d_lit, &ctx->d_target, &ctx->d_order,
                       &ctx->d_reads, &ctx->d_kidx, &ctx->d_frag, &ctx->d_state, &ctx->d_seq, &ctx->d_ops, &ctx->d_dcnt,
@@ -349,6 +350,41 @@ extern "C" int bb_upload_reference(bb_ctx *ctx, const uint8_t *bases, int64_t n_
     return BB_OK;
 }
 
+// The per-entry tables of a model (everything but the k-mer index) and the per-row summaries derived from them.
+static int upload_em_rows(bb_ctx *ctx, int k, int32_t n_rows, const int32_t *row_off, const double *cum,
+                          const uint8_t *flags, const uint32_t *slots, const uint8_t *pool, int64_t pool_len) {
+    const int64_t ne = row_off[n_rows];
+    int rc;
+    if ((rc = upload(ctx, ctx->em_rowoff, row_off, (size_t)n_rows + 1))) return rc;
+    if ((rc = upload(ctx, ctx->em_cum, cum, (size_t)ne))) return rc;
+    if ((rc = upload(ctx, ctx->em_flags, flags, (size_t)ne))) return rc;
+    if ((rc = upload(ctx, ctx->em_slots, slots, (size_t)ne * k))) return rc;
+    if ((rc = upload(ctx, ctx->em_pool, pool, (size_t)pool_len))) return rc;
+    std::vector<BBRowInfo> info((size_t)n_rows);
+    for (int32_t r = 0; r < n_rows; r++) {
+        const int32_t e0 = row_off[r], ne = row_off[r + 1] - e0;
+        if (ne <= 0) return set_err(ctx, BB_ERR_ARG, "error model: empty table row");
+        BBRowInfo &ri = info[(size_t)r];
+        ri.cum_last = cum[e0 + ne - 1]; ri.cum0 = cum[e0]; ri.e0 = e0; ri.ne = ne;
+        ri.first_is_identity = flags[e0] == 1 ? 1 : 0; ri.pad = 0;
+    }
+    if ((rc = upload(ctx, ctx->em_rowinfo, info.data(), info.size()))) return rc;
+    BB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // `info` is about to go out of scope
+    ctx->em.row_off = ctx->em_rowoff.as<int32_t>();
+    ctx->em.cum = ctx->em_cum.as<double>(); ctx->em.flags = ctx->em_flags.as<uint8_t>();
+    ctx->em.slots = ctx->em_slots.as<uint32_t>(); ctx->em.pool = ctx->em_pool.as<uint8_t>();
+    ctx->em.rowinfo = ctx->em_rowinfo.as<BBRowInfo>();
+    return BB_OK;
+}
+
+static void share_em(bb_ctx *ctx) {
+    ctx->have_em = true;
+    ctx->uploaded = false;
+    for (bb_ctx *kid : ctx->kids) {  // shared tables
+        kid->em = ctx->em; kid->em_hash = ctx->em_hash; kid->have_em = true; kid->uploaded = false;
+    }
+}
+
 extern "C" int bb_upload_error_model(bb_ctx *ctx, int k, int type, const int32_t *kmer_to_row, int64_t n_index,
                                      int32_t n_rows, const int32_t *row_off, const double *cum, const uint8_t *flags,
                                      const uint32_t *slots, const uint8_t *pool, int64_t pool_len) {
@@ -356,37 +392,40 @@ extern "C" int bb_upload_error_model(bb_ctx *ctx, int k, int type, const int32_t
     if (k < 1 || k > 12 || (type != 0 && type != 1)) return set_err(ctx, BB_ERR_ARG, "error model: k must be 1..12");
     BB_CUDA(ctx, cudaSetDevice(ctx->device));
     ctx->em = BBErrorModelDev{};
+    ctx->em_hash = BBEmHashDev{};
     ctx->em.k = k; ctx->em.type = type;
     if (type == 1) {
         if (!kmer_to_row || !row_off || !cum || !flags || !slots || n_rows <= 0 || n_index != (1ll << (2 * k)))
             return set_err(ctx, BB_ERR_ARG, "error model: missing tables");
-        const int64_t ne = row_off[n_rows];
         int rc;
         if ((rc = upload(ctx, ctx->em_k2r, kmer_to_row, (size_t)n_index))) return rc;
-        if ((rc = upload(ctx, ctx->em_rowoff, row_off, (size_t)n_rows + 1))) return rc;
-        if ((rc = upload(ctx, ctx->em_cum, cum, (size_t)ne))) return rc;
-        if ((rc = upload(ctx, ctx->em_flags, flags, (size_t)ne))) return rc;
-        if ((rc = upload(ctx, ctx->em_slots, slots, (size_t)ne * k))) return rc;
-        if ((rc = upload(ctx, ctx->em_pool, pool, (size_t)pool_len))) return rc;
-        std::vector<BBRowInfo> info((size_t)n_rows);
-        for (int32_t r = 0; r < n_rows; r++) {
-            const int32_t e0 = row_off[r], ne = row_off[r + 1] - e0;
-            if (ne <= 0) return set_err(ctx, BB_ERR_ARG, "error model: empty table row");
-            BBRowInfo &ri = info[(size_t)r];
-            ri.cum_last = cum[e0 + ne - 1]; ri.cum0 = cum[e0]; ri.e0 = e0; ri.ne = ne;
-            ri.first_is_identity = flags[e0] == 1 ? 1 : 0; ri.pad = 0;
-        }
-        if ((rc = upload(ctx, ctx->em_rowinfo, info.data(), info.size()))) return rc;
-        BB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // `info` is about to go out of scope
-        ctx->em.kmer_to_row = ctx->em_k2r.as<int32_t>(); ctx->em.row_off = ctx->em_rowoff.as<int32_t>();
-        ctx->em.cum = ctx->em_cum.as<double>(); ctx->em.flags = ctx->em_flags.as<uint8_t>();
-        ctx->em.slots = ctx->em_slots.as<uint32_t>(); ctx->em.pool = ctx->em_pool.as<uint8_t>();
-        ctx->em.rowinfo = ctx->em_rowinfo.as<BBRowInfo>();
+        if ((rc = upload_em_rows(ctx, k, n_rows, row_off, cum, flags, slots, pool, pool_len))) return rc;
+        ctx->em.kmer_to_row = ctx->em_k2r.as<int32_t>();
     }
     BB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    ctx->have_em = true;
-    ctx->uploaded = false;
-    for (bb_ctx *kid : ctx->kids) { kid->em = ctx->em; kid->have_em = true; kid->uploaded = false; }  // shared tables
+    share_em(ctx);
+    return BB_OK;
+}
+
+extern "C" int bb_upload_error_model_kmers(bb_ctx *ctx, int k, int32_t n_rows, const int64_t *kmer_codes,
+                                           const int32_t *row_off, const double *cum, const uint8_t *flags,
+                                           const uint32_t *slots, const uint8_t *pool, int64_t pool_len) {
+    if (!ctx) return BB_ERR_ARG;
+    if (!kmer_codes || !row_off || !cum || !flags || !slots || n_rows <= 0 || pool_len < 0 || (pool_len && !pool))
+        return set_err(ctx, BB_ERR_ARG, "error model: missing tables");
+    BBEmHashTable t;
+    std::string err;
+    if (!bb_build_em_hash(k, n_rows, kmer_codes, t, err)) return set_err(ctx, BB_ERR_ARG, err);
+    BB_CUDA(ctx, cudaSetDevice(ctx->device));
+    ctx->em = BBErrorModelDev{};
+    ctx->em_hash = BBEmHashDev{};
+    ctx->have_em = false;
+    int rc;
+    if ((rc = upload(ctx, ctx->em_hentries, t.entries.data(), t.entries.size()))) return rc;
+    if ((rc = upload_em_rows(ctx, k, n_rows, row_off, cum, flags, slots, pool, pool_len))) return rc;  // (synchronizes)
+    ctx->em.k = k; ctx->em.type = 1;
+    ctx->em_hash.entries = ctx->em_hentries.as<unsigned long long>(); ctx->em_hash.bits = t.bits;
+    share_em(ctx);
     return BB_OK;
 }
 
@@ -804,8 +843,11 @@ static int w_enqueue(bb_ctx *ctx) {
     ctx->marks.clear(); ctx->mark_used = 0;
     mark(ctx, st, "begin");
     BB_CUDA(ctx, cudaEventRecord(ctx->ev[0], st));
-    bb_k_build_fragments<<<n, 256, 0, st>>>(B, ctx->ref.as<uint8_t>(), ctx->em.k, ctx->seed,
-                                             ctx->em.type == 1 ? ctx->em.kmer_to_row : nullptr);
+    if (ctx->em.type == 1 && ctx->em_hash.entries)
+        bb_k_build_fragments<0, true><<<n, 256, 0, st>>>(B, ctx->ref.as<uint8_t>(), ctx->em.k, ctx->seed, nullptr, ctx->em_hash);
+    else
+        bb_k_build_fragments<<<n, 256, 0, st>>>(B, ctx->ref.as<uint8_t>(), ctx->em.k, ctx->seed,
+                                                 ctx->em.type == 1 ? ctx->em.kmer_to_row : nullptr);
     ctx->launches++;
     mark(ctx, st, "build_fragments");
     BB_CUDA(ctx, cudaEventRecord(ctx->ev[1], st));

@@ -12,9 +12,11 @@
 //   K6 bb_k_compact           seq[start_trim:-end_trim], qual likewise (simulate.py:355-356)
 #pragma once
 #include <cstdint>
+#include <type_traits>
 
 #include "../../include/badread_b200.h"
 #include "bb_align.cuh"
+#include "bb_em_tables.h"
 #include "bb_lane.cuh"
 #include "bb_qscore_tables.h"
 #include "bb_rng.cuh"
@@ -131,9 +133,12 @@ struct BBScratchPool {
 __constant__ uint8_t bb_c_comp[256];  // misc.REV_COMP_DICT, unknown -> 'N' (misc.py:56-67)
 
 // ------------------------------------------------------------------------------------------------ K1
-template <int BB_TU_ = 0>  // a template: only the translation unit that launches it compiles it
+// The k-mer index is the dense kmer_to_row[4^k] (k <= 12), or with HASH the open-addressing table `hash` of
+// bb_em_tables.h (any k up to 16); either one null: no index (the random model).
+template <int BB_TU_ = 0, bool HASH = false>  // a template: only the translation unit that launches it compiles it
 __global__ void __launch_bounds__(256) bb_k_build_fragments(BBBatchDev B, const uint8_t *__restrict__ ref, int k,
-                                                            unsigned long long seed, const int32_t *__restrict__ kmer_to_row) {
+                                                            unsigned long long seed, const int32_t *__restrict__ kmer_to_row,
+                                                            BBEmHashDev hash = BBEmHashDev{nullptr, 0}) {
     const int r = blockIdx.x;
     if (r >= B.n_reads) return;
     const BBReadDev rd = B.reads[r];
@@ -166,10 +171,10 @@ __global__ void __launch_bounds__(256) bb_k_build_fragments(BBBatchDev B, const 
     for (int x = threadIdx.x; x < flen; x += blockDim.x) { st[x] = BB_SLOT_NONE; ct[x] = 0u; }
     // match bitmap of the padded fragment (bb_build_peq layout), one ballot group per 32 bases
     __syncthreads();
-    if (kmer_to_row) {  // table row of every k-mer of the fragment: the loop looks a position up with one load
-        int *kx = B.kidx + rd.frag_off;
+    if (HASH ? hash.entries != nullptr : kmer_to_row != nullptr) {  // table row of every k-mer of the fragment: the
+        int *kx = B.kidx + rd.frag_off;                               // loop looks a position up with one load
         for (int x = threadIdx.x; x + k <= flen; x += blockDim.x) {
-            int idx = 0;
+            typename std::conditional<HASH, uint32_t, int>::type idx = 0;   // (a 16-mer's code needs all 32 bits)
             bool ok = true;
             for (int j = 0; j < k; j++) {
                 const uint8_t c = f[x + j];
@@ -177,7 +182,8 @@ __global__ void __launch_bounds__(256) bb_k_build_fragments(BBBatchDev B, const 
                 if (code < 0) ok = false;
                 idx = idx * 4 + (code & 3);
             }
-            kx[x] = ok ? kmer_to_row[idx] : -1;
+            if (HASH) kx[x] = ok ? bb_em_find(hash.entries, hash.bits, (uint32_t)idx) : -1;
+            else kx[x] = ok ? kmer_to_row[idx] : -1;
         }
     }
     uint4 *pq = B.fpeq + rd.fpeq_off;

@@ -167,7 +167,7 @@ bb_k_mutate(BBBatchDev B, BBErrorModelDev em, unsigned long long seed, int *work
 // results, but the serial part costs tens of nanoseconds per change instead of a global round trip.
 #define BB_MUT_IPT 2                                        // iterations per thread and step
 #define BB_MUT_ITERS (BB_WARPS_PER_CTA * 32 * BB_MUT_IPT)   // iterations per step
-#define BB_MUT_KMAX 16                                      // slots per candidate in shared memory (k <= 12)
+#define BB_MUT_KMAX 16                                      // slots per candidate in shared memory (k <= 16)
 #define BB_MUT_DIRTY_WORDS 128                              // bitmap over positions mod 4096
 
 template <int BB_TU_ = 0>  // a template: only the translation unit that launches it compiles it

@@ -2,7 +2,8 @@
 // bb_tu_models.cu.  Compiled for the host by the warp emulator as well (tests/emu).
 //   bbm_k_kmer_alternatives   badread error_model   (error_model.py:45-66: which read k-mers each reference k-mer became)
 //   bbm_k_cigar_qscores       badread qscore_model  (qscore_model.py:104-141: quality of the middle base per CIGAR window)
-// An alignment is a CTA, a window is a thread and a window's content is a 64-bit key in an open-addressing table: count,
+// An alignment is a CTA, a window is a thread and a window's content is a 64-bit key (128 bits for error-model k-mers
+// longer than 12: BBMTableWide) in an open-addressing table: count,
 // first occurrence (the reference's dicts keep insertion order, and its stable sorts break ties by it) and, for the qscore
 // model, a histogram of the 94 quality values.  Windows whose content does not fit a key go to an overflow list that the
 // host evaluates exactly.
@@ -10,6 +11,7 @@
 #include <cstdint>
 
 #define BBM_EMPTY 0xffffffffffffffffull
+#define BBM_WIDE_MAX_LEN 32   // read k-mer bases in the low word of a 128-bit key
 #define BBM_NQ 94   // quality characters '!' .. '~'
 
 struct BBMAln {
@@ -28,7 +30,28 @@ struct BBMTable {
     int *ovf_aln, *ovf_pos, *ovf_k;
     unsigned long long *n_ovf;
     long long ovf_cap;
+    static constexpr bool wide = false;
 };
+
+// Error-model key for 12 < k <= 16 (sm_90's 16-byte atomicCAS claims a slot): lo = read k-mer (2 bits a base from bit 0
+// up), hi = (reference k-mer << 6) | read k-mer length.  Empty: both words all ones (hi never is: the reference k-mer has
+// at most 32 bits).
+struct __align__(16) BBMKey128 { unsigned long long lo, hi; };
+
+struct BBMTableWide {   // BBMTable with 128-bit keys
+    BBMKey128 *keys;
+    unsigned long long *first;
+    unsigned int *counts;
+    long long cap;
+    int *status;
+    int *ovf_aln, *ovf_pos, *ovf_k;
+    unsigned long long *n_ovf;
+    long long ovf_cap;
+    static constexpr bool wide = true;
+};
+
+__device__ __forceinline__ bool bbm_is_empty(unsigned long long key) { return key == BBM_EMPTY; }
+__device__ __forceinline__ bool bbm_is_empty(const BBMKey128 &key) { return key.lo == BBM_EMPTY && key.hi == BBM_EMPTY; }
 
 __device__ __forceinline__ unsigned long long bbm_mix64(unsigned long long x) {
     x ^= x >> 33; x *= 0xff51afd7ed558ccdull; x ^= x >> 33; x *= 0xc4ceb9fe1a85ec53ull; x ^= x >> 33;
@@ -51,7 +74,25 @@ __device__ long long bbm_table_slot(const BBMTable &T, unsigned long long key) {
     return -1;
 }
 
-__device__ void bbm_overflow(const BBMTable &T, int aln, int pos, int k) {
+// The same for a 128-bit key (Table = BBMTableWide).  A template, so that code which never counts wide keys (the warp
+// emulator's other harnesses) needs no 16-byte atomicCAS.
+template <typename Table>
+__device__ long long bbm_table_slot(const Table &T, BBMKey128 key) {
+    if (*(volatile int *)&T.status[0]) return -1;
+    unsigned long long h = bbm_mix64(key.hi ^ bbm_mix64(key.lo)) & (unsigned long long)(T.cap - 1);
+    const long long limit = T.cap < 1024 ? T.cap : 1024;
+    const BBMKey128 empty{BBM_EMPTY, BBM_EMPTY};
+    for (long long probe = 0; probe < limit; probe++) {
+        const BBMKey128 prev = atomicCAS(&T.keys[h], empty, key);
+        if (bbm_is_empty(prev) || (prev.lo == key.lo && prev.hi == key.hi)) return (long long)h;
+        h = (h + 1) & (unsigned long long)(T.cap - 1);
+    }
+    atomicExch(&T.status[0], 1);
+    return -1;
+}
+
+template <typename Table>
+__device__ void bbm_overflow(const Table &T, int aln, int pos, int k) {
     const unsigned long long i = atomicAdd(T.n_ovf, 1ull);
     if ((long long)i < T.ovf_cap) { T.ovf_aln[i] = aln; T.ovf_pos[i] = pos; T.ovf_k[i] = k; }
     else atomicExch(&T.status[1], 1);
@@ -64,8 +105,10 @@ __device__ __forceinline__ int bbm_base_code(uint8_t c) { return c == 'A' ? 0 : 
 // to the column of reference base r + k - 1; its read k-mer is read[rp[r] : rp[r+k-1] + isM[r+k-1]) with rp[x] = read
 // bases in front of x's column (the first window starts at column 0, i.e. at read base 0, whatever the alignment starts
 // with).  Counted if the read k-mer has more than one base, both k-mers are ACGT only and they agree in their first and
-// last base.  Key: reference k-mer (2k bits) | length (6 bits) | read k-mer (2 bits a base).
-__global__ void __launch_bounds__(256) bbm_k_kmer_alternatives(BBMAln A, int n_aln, int k, int *rp_pool, uint8_t *ism_pool, BBMTable T) {
+// last base.  Key: reference k-mer (2k bits) | length (6 bits) | read k-mer (2 bits a base); with a BBMTableWide
+// (12 < k <= 16) the BBMKey128 of the same three fields.
+template <typename Table>
+__global__ void __launch_bounds__(256) bbm_k_kmer_alternatives(BBMAln A, int n_aln, int k, int *rp_pool, uint8_t *ism_pool, Table T) {
     const int a = blockIdx.x;
     if (a >= n_aln) return;
     const uint8_t *read = A.read + A.read_off[a], *ref = A.ref + A.ref_off[a];
@@ -79,7 +122,7 @@ __global__ void __launch_bounds__(256) bbm_k_kmer_alternatives(BBMAln A, int n_a
         else if (type == 2) for (int i = 0; i < len; i++) { rp[r0 + i] = p0; ism[r0 + i] = 0; }
     }
     __syncthreads();
-    const int shift_ref = 64 - 2 * k, shift_len = shift_ref - 6, max_len = shift_len / 2;
+    const int shift_ref = 64 - 2 * k, shift_len = shift_ref - 6, max_len = Table::wide ? BBM_WIDE_MAX_LEN : shift_len / 2;
     for (int r = threadIdx.x; r + k <= n_ref; r += blockDim.x) {
         const int p_lo = r == 0 ? 0 : rp[r], p_hi = rp[r + k - 1] + ism[r + k - 1];
         const int len = p_hi - p_lo;
@@ -93,7 +136,7 @@ __global__ void __launch_bounds__(256) bbm_k_kmer_alternatives(BBMAln A, int n_a
             key = (key << 2) | (unsigned long long)(c & 3);
         }
         if (!ok) continue;
-        key <<= shift_ref;
+        if (!Table::wide) key <<= shift_ref;
         if (len > max_len) {  // (the host checks the read k-mer's alphabet itself)
             bbm_overflow(T, a, r, k);
             continue;
@@ -105,8 +148,12 @@ __global__ void __launch_bounds__(256) bbm_k_kmer_alternatives(BBMAln A, int n_a
             rb |= (unsigned long long)(c & 3) << (2 * j);
         }
         if (!ok) continue;
-        key |= ((unsigned long long)len << shift_len) | rb;
-        const long long s = bbm_table_slot(T, key);
+        long long s;
+        if constexpr (Table::wide) s = bbm_table_slot(T, BBMKey128{rb, (key << 6) | (unsigned long long)len});
+        else {
+            key |= ((unsigned long long)len << shift_len) | rb;
+            s = bbm_table_slot(T, key);
+        }
         if (s < 0) return;
         atomicAdd(&T.counts[s], 1u);
         atomicMin(&T.first[s], ((unsigned long long)a << 32) | (unsigned long long)r);
@@ -170,10 +217,11 @@ __global__ void __launch_bounds__(256) bbm_k_cigar_qscores(BBMAln A, int n_aln, 
 }
 
 // Occupied slots -> dense output (arbitrary order; the host sorts by first occurrence).
-__global__ void bbm_k_compact(BBMTable T, int per_slot, unsigned long long *keys_out, unsigned long long *first_out,
+template <typename Table, typename Key>
+__global__ void bbm_k_compact(Table T, int per_slot, Key *keys_out, unsigned long long *first_out,
                           unsigned int *counts_out, unsigned long long *n_out, long long out_cap) {
     const long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= T.cap || T.keys[s] == BBM_EMPTY) return;
+    if (s >= T.cap || bbm_is_empty(T.keys[s])) return;
     const unsigned long long i = atomicAdd(n_out, 1ull);
     if ((long long)i >= out_cap) return;
     keys_out[i] = T.keys[s];

@@ -1,5 +1,6 @@
 // bb_tu_models.cu — the counting passes of the model builders on the GPU (SURVEY.md 8f row f4):
 //   bb_count_kmer_alternatives   badread error_model   (error_model.py:31-83: which read k-mers each reference k-mer became)
+//   bb_count_kmer_alternatives_wide   the same for 12 < k <= 16, with 128-bit keys
 //   bb_count_cigar_qscores       badread qscore_model  (qscore_model.py:78-153: quality of the middle base per CIGAR window)
 // The reference walks every alignment column by column in Python, rebuilding a window string per step; here an
 // alignment is a CTA, a window is a thread and a (window content) is a 64-bit key in an open-addressing table:
@@ -42,7 +43,7 @@ struct DevMem {   // everything a call allocates, released on every exit path
 
 thread_local char g_model_error[256] = "";
 
-int count_common(bool qscores, int device, int k, int max_del, int32_t n_aln, const uint8_t *read, const uint8_t *qual,
+int count_common(bool qscores, bool wide, int device, int k, int max_del, int32_t n_aln, const uint8_t *read, const uint8_t *qual,
                  const int64_t *read_off, const uint8_t *ref, const int64_t *ref_off, const uint32_t *ops, const int32_t *op_read0,
                  const int32_t *op_ref0, const int64_t *ops_off, int64_t table_cap, uint64_t *keys_out, uint64_t *first_out,
                  uint32_t *counts_out, int64_t *n_entries, uint64_t *overall_out, int64_t ovf_cap, int32_t *ovf_aln,
@@ -50,7 +51,8 @@ int count_common(bool qscores, int device, int k, int max_del, int32_t n_aln, co
     g_model_error[0] = 0;
     if (n_aln <= 0 || !read || !read_off || !ref || !ref_off || !ops || !ops_off || !op_read0 || !op_ref0 || !keys_out ||
         !first_out || !counts_out || !n_entries || !n_ovf || table_cap < 16 || (table_cap & (table_cap - 1)) ||
-        (qscores && (!qual || !overall_out || k < 1 || k > 13 || !(k & 1) || max_del < 0)) || (!qscores && (k < 1 || k > 12))) {
+        (qscores && (!qual || !overall_out || k < 1 || k > 13 || !(k & 1) || max_del < 0)) ||
+        (!qscores && !wide && (k < 1 || k > 12)) || (wide && (k <= 12 || k > 16))) {
         std::snprintf(g_model_error, sizeof(g_model_error), "bb_count_*: invalid argument");
         return BB_ERR_ARG;
     }
@@ -61,6 +63,7 @@ int count_common(bool qscores, int device, int k, int max_del, int32_t n_aln, co
     (void)cudaGetLastError();
     const int64_t n_read = read_off[n_aln], n_ref = ref_off[n_aln], n_ops = ops_off[n_aln];
     const int per_slot = qscores ? BBM_NQ : 1;
+    const size_t key_bytes = wide ? sizeof(BBMKey128) : 8;
     DevMem mem;
     BBMAln A{};
     uint8_t *d_read, *d_qual = nullptr, *d_ref;
@@ -80,7 +83,8 @@ int count_common(bool qscores, int device, int k, int max_del, int32_t n_aln, co
     A.ops = d_ops; A.op_read0 = d_p0; A.op_ref0 = d_r0;
     BBMTable T{};
     T.cap = table_cap; T.ovf_cap = ovf_cap;
-    BBM_TRY(mem.get(&T.keys, (size_t)table_cap * 8, nullptr, 0xff));
+    if (wide) BBM_TRY(mem.get(&T.keys, 16, nullptr, 0xff));   // (unused: the 128-bit keys are TW's)
+    else BBM_TRY(mem.get(&T.keys, (size_t)table_cap * 8, nullptr, 0xff));
     BBM_TRY(mem.get(&T.first, (size_t)table_cap * 8, nullptr, 0xff));
     BBM_TRY(mem.get(&T.counts, (size_t)table_cap * per_slot * 4, nullptr, 0));
     BBM_TRY(mem.get(&T.status, 16, nullptr, 0));
@@ -88,6 +92,12 @@ int count_common(bool qscores, int device, int k, int max_del, int32_t n_aln, co
     BBM_TRY(mem.get(&T.ovf_aln, (size_t)ovf_cap * 4));
     BBM_TRY(mem.get(&T.ovf_pos, (size_t)ovf_cap * 4));
     BBM_TRY(mem.get(&T.ovf_k, (size_t)ovf_cap * 4));
+    BBMTableWide TW{};
+    if (wide) {
+        TW.first = T.first; TW.counts = T.counts; TW.cap = T.cap; TW.status = T.status;
+        TW.ovf_aln = T.ovf_aln; TW.ovf_pos = T.ovf_pos; TW.ovf_k = T.ovf_k; TW.n_ovf = T.n_ovf; TW.ovf_cap = T.ovf_cap;
+        BBM_TRY(mem.get(&TW.keys, (size_t)table_cap * sizeof(BBMKey128), nullptr, 0xff));
+    }
     unsigned long long *d_overall = nullptr;
     if (qscores) {
         uint8_t *sym; int *dc, *lead;
@@ -100,16 +110,19 @@ int count_common(bool qscores, int device, int k, int max_del, int32_t n_aln, co
         int *rp; uint8_t *ism;
         BBM_TRY(mem.get(&rp, (size_t)n_ref * 4));
         BBM_TRY(mem.get(&ism, (size_t)n_ref));
-        bbm_k_kmer_alternatives<<<n_aln, 256>>>(A, n_aln, k, rp, ism, T);
+        if (wide) bbm_k_kmer_alternatives<<<n_aln, 256>>>(A, n_aln, k, rp, ism, TW);
+        else bbm_k_kmer_alternatives<<<n_aln, 256>>>(A, n_aln, k, rp, ism, T);
     }
     BBM_TRY(cudaGetLastError());
     unsigned long long *d_keys_out, *d_first_out, *d_n;
     unsigned int *d_counts_out;
-    BBM_TRY(mem.get(&d_keys_out, (size_t)table_cap * 8));
+    BBM_TRY(mem.get(&d_keys_out, (size_t)table_cap * key_bytes));
     BBM_TRY(mem.get(&d_first_out, (size_t)table_cap * 8));
     BBM_TRY(mem.get(&d_counts_out, (size_t)table_cap * per_slot * 4));
     BBM_TRY(mem.get(&d_n, 16, nullptr, 0));
-    bbm_k_compact<<<(unsigned int)((table_cap + 255) / 256), 256>>>(T, per_slot, d_keys_out, d_first_out, d_counts_out, d_n, table_cap);
+    const unsigned int n_blocks = (unsigned int)((table_cap + 255) / 256);
+    if (wide) bbm_k_compact<<<n_blocks, 256>>>(TW, per_slot, (BBMKey128 *)d_keys_out, d_first_out, d_counts_out, d_n, table_cap);
+    else bbm_k_compact<<<n_blocks, 256>>>(T, per_slot, d_keys_out, d_first_out, d_counts_out, d_n, table_cap);
     BBM_TRY(cudaGetLastError());
     int status[2] = {0, 0};
     unsigned long long n = 0, novf = 0;
@@ -121,7 +134,7 @@ int count_common(bool qscores, int device, int k, int max_del, int32_t n_aln, co
         std::snprintf(g_model_error, sizeof(g_model_error), "bb_count_*: %s too small", status[0] ? "table" : "overflow list");
         return BB_ERR_CAPACITY;
     }
-    BBM_TRY(cudaMemcpy(keys_out, d_keys_out, (size_t)n * 8, cudaMemcpyDeviceToHost));
+    BBM_TRY(cudaMemcpy(keys_out, d_keys_out, (size_t)n * key_bytes, cudaMemcpyDeviceToHost));
     BBM_TRY(cudaMemcpy(first_out, d_first_out, (size_t)n * 8, cudaMemcpyDeviceToHost));
     BBM_TRY(cudaMemcpy(counts_out, d_counts_out, (size_t)n * per_slot * 4, cudaMemcpyDeviceToHost));
     if (novf) {
@@ -143,7 +156,17 @@ extern "C" int bb_count_kmer_alternatives(int device, int k, int32_t n_aln, cons
                                           int64_t table_cap, uint64_t *keys_out, uint64_t *first_out, uint32_t *counts_out,
                                           int64_t *n_entries, int64_t ovf_cap, int32_t *ovf_aln, int32_t *ovf_pos,
                                           int32_t *ovf_k, int64_t *n_ovf) {
-    return count_common(false, device, k, 0, n_aln, read, nullptr, read_off, ref, ref_off, ops, op_read0, op_ref0, ops_off,
+    return count_common(false, false, device, k, 0, n_aln, read, nullptr, read_off, ref, ref_off, ops, op_read0, op_ref0, ops_off,
+                        table_cap, keys_out, first_out, counts_out, n_entries, nullptr, ovf_cap, ovf_aln, ovf_pos, ovf_k, n_ovf);
+}
+
+extern "C" int bb_count_kmer_alternatives_wide(int device, int k, int32_t n_aln, const uint8_t *read, const int64_t *read_off,
+                                               const uint8_t *ref, const int64_t *ref_off, const uint32_t *ops,
+                                               const int32_t *op_read0, const int32_t *op_ref0, const int64_t *ops_off,
+                                               int64_t table_cap, uint64_t *keys_out, uint64_t *first_out, uint32_t *counts_out,
+                                               int64_t *n_entries, int64_t ovf_cap, int32_t *ovf_aln, int32_t *ovf_pos,
+                                               int32_t *ovf_k, int64_t *n_ovf) {
+    return count_common(false, true, device, k, 0, n_aln, read, nullptr, read_off, ref, ref_off, ops, op_read0, op_ref0, ops_off,
                         table_cap, keys_out, first_out, counts_out, n_entries, nullptr, ovf_cap, ovf_aln, ovf_pos, ovf_k, n_ovf);
 }
 
@@ -153,7 +176,7 @@ extern "C" int bb_count_cigar_qscores(int device, int k, int max_del, int32_t n_
                                       int64_t table_cap, uint64_t *keys_out, uint64_t *first_out, uint32_t *counts_out,
                                       int64_t *n_entries, uint64_t *overall_out, int64_t ovf_cap, int32_t *ovf_aln,
                                       int32_t *ovf_pos, int32_t *ovf_k, int64_t *n_ovf) {
-    return count_common(true, device, k, max_del, n_aln, read, qual, read_off, ref, ref_off, ops, op_read0, op_ref0, ops_off,
+    return count_common(true, false, device, k, max_del, n_aln, read, qual, read_off, ref, ref_off, ops, op_read0, op_ref0, ops_off,
                         table_cap, keys_out, first_out, counts_out, n_entries, overall_out, ovf_cap, ovf_aln, ovf_pos, ovf_k,
                         n_ovf);
 }

@@ -155,15 +155,28 @@ class Engine(object):
         self._ref_keepalive = arr
         self._check(self._lib.bb_upload_reference(self._ctx, _ptr(arr), arr.size), 'bb_upload_reference')
 
-    def set_error_model(self, error_model):
+    def set_error_model(self, error_model, index='auto'):
+        """index: how the device finds a k-mer's row.  'auto': the dense kmer_to_row[4^k] when the model has one
+        (k <= 12), else a hash table of the rows' k-mers; 'hash': the hash table for any k (same reads, for tests and
+        measurement)."""
+        if index not in ('auto', 'hash'):
+            raise ValueError(f"index must be 'auto' or 'hash', not {index!r}")
         t = error_model.to_device_tables()
         if t['type'] == 0:
             rc = self._lib.bb_upload_error_model(self._ctx, 1, 0, None, 0, 0, None, None, None, None, None, 0)
-        else:
+            name = 'bb_upload_error_model'
+        elif index == 'auto' and t['index'] == 'dense':
             rc = self._lib.bb_upload_error_model(self._ctx, t['k'], 1, _ptr(t['kmer_to_row']), t['kmer_to_row'].size,
                                                  len(t['row_off']) - 1, _ptr(t['row_off']), _ptr(t['cum']),
                                                  _ptr(t['flags']), _ptr(t['slots']), _ptr(t['pool']), t['pool'].size)
-        self._check(rc, 'bb_upload_error_model')
+            name = 'bb_upload_error_model'
+        else:
+            codes = np.ascontiguousarray(t['kmer_codes'], dtype=np.int64)
+            rc = self._lib.bb_upload_error_model_kmers(self._ctx, t['k'], len(t['row_off']) - 1, _ptr(codes),
+                                                       _ptr(t['row_off']), _ptr(t['cum']), _ptr(t['flags']),
+                                                       _ptr(t['slots']), _ptr(t['pool']), t['pool'].size)
+            name = 'bb_upload_error_model_kmers'
+        self._check(rc, name)
         self.error_model = error_model
 
     def set_qscore_model(self, qscore_model):

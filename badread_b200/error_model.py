@@ -6,7 +6,10 @@ ErrorModel - host side of the k-mer error model, same plugin surface as
 
 Table layout (shared by the CUDA path and the CPU oracle):
   kmer_to_row[4^k]  row of each ACGT k-mer, -1 if the model has no line for it (then: one random change,
-                    error_model.py:143-144; the same happens for k-mers holding non-ACGT characters)
+                    error_model.py:143-144; the same happens for k-mers holding non-ACGT characters).  Only for
+                    k <= DENSE_MAX_K: larger models (up to MAX_K) are indexed by `kmer_codes` alone, which the library
+                    turns into a hash table (bb_upload_error_model_kmers)
+  kmer_codes[n_rows] the 2-bit code of each row's k-mer (base j in bits 2*(k-1-j), A C G T = 0 1 2 3)
   row_off[n_rows+1] entry range of each row
   per entry:        cum    list(itertools.accumulate(probs)) - what random.choices builds (error_model.py:156)
                     flags  bit0: ''.join(alt) == kmer (the `continue` at simulate.py:300)
@@ -37,7 +40,8 @@ from .misc import get_open_func, get_random_base, get_random_different_base, ran
 BUILTIN_MODELS = ('nanopore2018', 'nanopore2020', 'nanopore2023', 'pacbio2016', 'pacbio2021')
 MODEL_DIR = pathlib.Path(os.path.dirname(os.path.realpath(__file__))) / 'models'
 _CODE = {'A': 0, 'C': 1, 'G': 2, 'T': 3}
-MAX_K = 12
+DENSE_MAX_K = 12   # largest k with a dense kmer_to_row[4^k] (64 MB at k = 12)
+MAX_K = 16         # a k-mer's code fits 32 bits; the mutate kernel keeps 16 slots per candidate in shared memory
 
 
 def _ptr(a):
@@ -84,7 +88,7 @@ class ErrorModel(object):
         with np.load(str(path)) as z:
             self.kmer_size = int(z['k'])
             self._tables = {key: np.ascontiguousarray(z[key]) for key in
-                            ('kmer_to_row', 'row_off', 'cum', 'flags', 'slots', 'pool', 'probs', 'kmer_codes')}
+                            ('kmer_to_row', 'row_off', 'cum', 'flags', 'slots', 'pool', 'probs', 'kmer_codes') if key in z}
         print(f'\r  done: loaded error distributions for {len(self._tables["row_off"]) - 1} '
               f'{self.kmer_size}-mers', file=output)
 
@@ -112,7 +116,7 @@ class ErrorModel(object):
             sys.exit('Error: the error model file holds no k-mers')
         assert k > 2  # error_model.py:188
         if k > MAX_K:
-            sys.exit(f'Error: error models with k > {MAX_K} are not supported by badread_b200')
+            sys.exit(f'Error: error models with k > {MAX_K} are not supported by badread_b200 (this model has k = {k})')
         kmers = list(rows.keys())
         for kmer in kmers:
             if any(c not in _CODE for c in kmer):
@@ -145,7 +149,7 @@ class ErrorModel(object):
         assert sys.version_info >= (3, 12), 'the static remainder entry assumes CPython >= 3.12 (compensated sum())'
         row_off = [0]
         cum, flags, slot_rows, probs_flat = [], [], [], []
-        kmer_to_row = np.full(4 ** k, -1, dtype=np.int32)
+        kmer_to_row = np.full(4 ** k, -1, dtype=np.int32) if k <= DENSE_MAX_K else None
         kmer_codes = np.zeros(len(kmers), dtype=np.int64)
         a = 0
         for r, kmer in enumerate(kmers):
@@ -167,10 +171,10 @@ class ErrorModel(object):
             code = 0
             for c in kmer:
                 code = code * 4 + _CODE[c]
-            kmer_to_row[code] = r
+            if kmer_to_row is not None:
+                kmer_to_row[code] = r
             kmer_codes[r] = code
         self._tables = {
-            'kmer_to_row': kmer_to_row,
             'row_off': np.asarray(row_off, dtype=np.int32),
             'cum': np.asarray(cum, dtype=np.float64),
             'flags': np.asarray(flags, dtype=np.uint8),
@@ -179,6 +183,8 @@ class ErrorModel(object):
             'probs': np.asarray(probs_flat, dtype=np.float64),
             'kmer_codes': kmer_codes,
         }
+        if kmer_to_row is not None:
+            self._tables['kmer_to_row'] = kmer_to_row
 
     def save_tables(self, path):
         t = self._tables
@@ -186,12 +192,15 @@ class ErrorModel(object):
 
     # ------------------------------------------------------------------------------------------ surface
     def to_device_tables(self):
-        """Flat arrays for bb_upload_error_model / the oracle. 'random' has no tables."""
+        """Flat arrays for bb_upload_error_model(_kmers) / the oracle. 'random' has no tables.  `index` says how the
+        k-mers are found: 'dense' (kmer_to_row[4^k], k <= 12) or 'hash' (kmer_codes only, for the library's hash
+        table)."""
         if self.type == 'random':
-            return {'k': 1, 'type': 0}
+            return {'k': 1, 'type': 0, 'index': None}
         t = dict(self._tables)
         t['k'] = self.kmer_size
         t['type'] = 1
+        t['index'] = 'dense' if 'kmer_to_row' in t else 'hash'
         return t
 
     def _kmer_of_row(self, r):

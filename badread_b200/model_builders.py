@@ -194,15 +194,18 @@ def _ptr(a):
 
 
 def _count(which, flat, k, max_del=0, device=0):
-    """Runs bb_count_kmer_alternatives / bb_count_cigar_qscores, growing the table until it fits."""
+    """Runs bb_count_kmer_alternatives ('kmers'), bb_count_kmer_alternatives_wide ('kmers_wide': keys come back as
+    (n, 2) words, read k-mer and reference k-mer << 6 | length) or bb_count_cigar_qscores ('cigars'), growing the table
+    until it fits."""
     L = _lib.lib()
-    per_slot = 1 if which == 'kmers' else N_Q
+    per_slot = N_Q if which == 'cigars' else 1
+    key_words = 2 if which == 'kmers_wide' else 1
     cap = 1 << 18       # slots; doubled until the distinct keys fit (k-mer pairs: at most one per window)
-    while which == 'kmers' and cap < min(2 * int(flat.ref_off[-1]) + 16, 1 << 22):
+    while which != 'cigars' and cap < min(2 * int(flat.ref_off[-1]) + 16, 1 << 22):
         cap <<= 1
     ovf_cap = 1 << 16
     while True:
-        keys = np.empty(cap, dtype=np.uint64); first = np.empty(cap, dtype=np.uint64)
+        keys = np.empty(cap * key_words, dtype=np.uint64); first = np.empty(cap, dtype=np.uint64)
         counts = np.empty(cap * per_slot, dtype=np.uint32)
         ovf = [np.empty(ovf_cap, dtype=np.int32) for _ in range(3)]
         overall = np.zeros(N_Q, dtype=np.uint64)
@@ -212,6 +215,8 @@ def _count(which, flat, k, max_del=0, device=0):
         tail = [ovf_cap, _ptr(ovf[0]), _ptr(ovf[1]), _ptr(ovf[2]), ctypes.byref(n_ovf)]
         if which == 'kmers':
             rc = L.bb_count_kmer_alternatives(device, k, flat.n, _ptr(flat.read), _ptr(flat.read_off), *common, *tail)
+        elif which == 'kmers_wide':
+            rc = L.bb_count_kmer_alternatives_wide(device, k, flat.n, _ptr(flat.read), _ptr(flat.read_off), *common, *tail)
         else:
             rc = L.bb_count_cigar_qscores(device, k, max_del, flat.n, _ptr(flat.read), _ptr(flat.qual), _ptr(flat.read_off),
                                           *common, _ptr(overall), *tail)
@@ -224,23 +229,18 @@ def _count(which, flat, k, max_del=0, device=0):
         if rc != _lib.BB_OK:
             raise RuntimeError('model builder: ' + L.bb_model_error().decode(errors='replace'))
         n, m = int(n_entries.value), int(n_ovf.value)
-        return keys[:n], first[:n], counts[:n * per_slot].reshape(n, per_slot), overall, [o[:m] for o in ovf]
+        keys = keys[:n * key_words].reshape(n, 2) if key_words == 2 else keys[:n]
+        return keys, first[:n], counts[:n * per_slot].reshape(n, per_slot), overall, [o[:m] for o in ovf]
 
 
 # ---------------------------------------------------------------------------------------------------- error model
-def make_error_model(args, output=sys.stderr, dot_interval=1000):
-    """error_model.py:31-83."""
-    refs = load_fasta(args.reference)[0]
-    reads = load_fastq(args.reads, output=output)
-    alignments = load_alignments(args.alignment, args.max_alignments, output=output)
-    if len(alignments) == 0:
-        sys.exit('Error: no usable alignments')
-    k = args.k_size
-    flat = FlatAlignments(alignments, reads, refs, output, dot_interval)
-    keys, first, counts, _, ovf = _count('kmers', flat, k)
-    counts = counts[:, 0].astype(np.int64)
-    shift_ref, shift_len = np.uint64(64 - 2 * k), np.uint64(58 - 2 * k)
-    # read k-mers too long for a key (the overflow list): counted here, exactly; {reference k-mer: {read k-mer: [count, first]}}
+MAX_K_DENSE = 12    # 64-bit keys and dense per-k-mer arrays (4^k entries)
+MAX_K_WIDE = 16     # 128-bit keys, aggregated over the reference k-mers that occur
+
+
+def _overflow_alternatives(flat, ovf, k):
+    """Read k-mers too long for a key (the overflow list), counted here, exactly:
+    {reference k-mer code: {read k-mer: [count, first occurrence]}}."""
     long_alts, cache = collections.defaultdict(dict), {}
     for a, r, _ in zip(*(o.tolist() for o in ovf)):
         if a not in cache:
@@ -256,6 +256,76 @@ def make_error_model(args, output=sys.stderr, dot_interval=1000):
             entry = long_alts[code].setdefault(read_kmer, [0, (a << 32) | r])
             entry[0] += 1
             entry[1] = min(entry[1], (a << 32) | r)
+    return long_alts
+
+
+def _error_model_lines_sparse(args, flat, k):
+    """The model file for 12 < k <= 16 from 128-bit keys: the same lines as the dense path below, aggregated over the
+    reference k-mers that occur (np.unique) instead of arrays of 4^k entries."""
+    keys, first, counts, _, ovf = _count('kmers_wide', flat, k)
+    counts = counts[:, 0].astype(np.int64)
+    read_bits, hi = keys[:, 0], keys[:, 1]
+    refcode = (hi >> np.uint64(6)).astype(np.int64)
+    lens = (hi & np.uint64(63)).astype(np.int64)
+    long_alts = _overflow_alternatives(flat, ovf, k)
+    codes = np.unique(np.concatenate([refcode, np.fromiter(long_alts, dtype=np.int64, count=len(long_alts))]))
+    group_of = np.searchsorted(codes, refcode)            # entry -> index of its reference k-mer in `codes`
+    totals = np.bincount(group_of, weights=counts, minlength=codes.size).astype(np.int64)
+    for code, alts in long_alts.items():
+        totals[np.searchsorted(codes, code)] += sum(c for c, _ in alts.values())
+    same = np.zeros(refcode.size, dtype=np.uint64)        # the read bits of the unchanged k-mer: base j at bits 2j
+    rc = refcode.astype(np.uint64)
+    for j in range(k):
+        same |= ((rc >> np.uint64(2 * (k - 1 - j))) & np.uint64(3)) << np.uint64(2 * j)
+    is_identity = (lens == k) & (read_bits == same)
+    unchanged = np.zeros(codes.size, dtype=np.int64)
+    unchanged[group_of[is_identity]] = counts[is_identity]
+    alt = np.flatnonzero(~is_identity)
+    order = alt[np.lexsort((first[alt], -counts[alt], refcode[alt]))]
+    group = refcode[order]
+    starts = np.flatnonzero(np.concatenate([[True], group[1:] != group[:-1]])) if order.size else np.zeros(0, dtype=np.int64)
+    rank = np.arange(order.size) - np.repeat(starts, np.diff(np.concatenate([starts, [order.size]])))
+    # (a reference k-mer with alternatives in the overflow list keeps all of its entries: they are merged below)
+    crowded = np.isin(group, np.fromiter(long_alts, dtype=np.int64, count=len(long_alts)))
+    kept = order[(rank < args.max_alt) | crowded]
+    kept_lens = lens[kept]
+    width = int(kept_lens.max()) if kept.size else 1
+    letters = np.frombuffer(b'ACGT', dtype=np.uint8)[((read_bits[kept][:, None] >> (np.uint64(2) * np.arange(width, dtype=np.uint64))) &
+                                                    np.uint64(3)).astype(np.int64)].tobytes()
+    kept_code, kept_count, kept_first = refcode[kept].tolist(), counts[kept].tolist(), first[kept].tolist()
+    per_code = collections.defaultdict(list)
+    for i, n in enumerate(kept_lens.tolist()):
+        per_code[kept_code[i]].append((letters[i * width:i * width + n].decode(), kept_count[i], kept_first[i]))
+    out = []
+    for code, total, n_same in zip(codes.tolist(), totals.tolist(), unchanged.tolist()):
+        kmer = ''.join('ACGT'[(code >> (2 * (k - 1 - j))) & 3] for j in range(k))
+        alts = per_code.get(code, [])
+        if code in long_alts:
+            alts = sorted(alts + [(a, c, s) for a, (c, s) in long_alts[code].items()], key=lambda x: (-x[1], x[2]))
+        line = [f'{kmer},{n_same / total:.6f};']
+        line.extend(f'{a},{c / total:.6f};' for a, c, _ in alts[:args.max_alt])
+        out.append(''.join(line))
+    return '\n'.join(out)
+
+
+def make_error_model(args, output=sys.stderr, dot_interval=1000):
+    """error_model.py:31-83."""
+    refs = load_fasta(args.reference)[0]
+    reads = load_fastq(args.reads, output=output)
+    alignments = load_alignments(args.alignment, args.max_alignments, output=output)
+    if len(alignments) == 0:
+        sys.exit('Error: no usable alignments')
+    k = args.k_size
+    if k > MAX_K_WIDE:
+        sys.exit(f'Error: error models with k > {MAX_K_WIDE} are not supported by badread_b200')
+    flat = FlatAlignments(alignments, reads, refs, output, dot_interval)
+    if k > MAX_K_DENSE:
+        print(_error_model_lines_sparse(args, flat, k))
+        return
+    keys, first, counts, _, ovf = _count('kmers', flat, k)
+    counts = counts[:, 0].astype(np.int64)
+    shift_ref, shift_len = np.uint64(64 - 2 * k), np.uint64(58 - 2 * k)
+    long_alts = _overflow_alternatives(flat, ovf, k)
     # per reference k-mer: total, the count of the unchanged k-mer, and the alternatives by (count, first occurrence) -
     # the order of the reference's stable sort by fraction over its insertion-ordered dict
     refcode = (keys >> shift_ref).astype(np.int64)

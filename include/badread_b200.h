@@ -94,6 +94,14 @@ BB_API int bb_upload_error_model(bb_ctx *ctx, int k, int type, const int32_t *km
                           const int32_t *row_off, const double *cum, const uint8_t *flags, const uint32_t *slots,
                           const uint8_t *pool, int64_t pool_len);
 
+/* The same tables with the k-mer index as a hash table instead of kmer_to_row[4^k], for any k in 3..16 (k > 12 has no
+ *  dense form): row r has the k-mer whose 2-bit code (base j in bits 2*(k-1-j), A C G T = 0 1 2 3) is kmer_codes[r].  A
+ *  k-mer without a row, or one holding a non-ACGT base, gets one random change, as with the dense index.  A code outside
+ *  0 .. 4^k-1 or one that two rows share is rejected (BB_ERR_ARG, message in bb_last_error). */
+BB_API int bb_upload_error_model_kmers(bb_ctx *ctx, int k, int32_t n_rows, const int64_t *kmer_codes, const int32_t *row_off,
+                                const double *cum, const uint8_t *flags, const uint32_t *slots, const uint8_t *pool,
+                                int64_t pool_len);
+
 /* Qscore model tables (flat form of QScoreModel.scores / .probabilities, qscore_model.py:178-271).
  *  Key i is the CIGAR string key_chars[key_off[i] .. key_off[i+1]) over {=,X,I,D}, of any length;
  *  row_off[n_keys+1]; scores / cum per entry. kmer_size as QScoreModel.kmer_size.  A repeated key keeps its last row
@@ -291,6 +299,14 @@ BB_API int bb_count_kmer_alternatives(int device, int k, int32_t n_aln, const ui
                                const int32_t *op_ref0, const int64_t *ops_off, int64_t table_cap, uint64_t *keys_out,
                                uint64_t *first_out, uint32_t *counts_out, int64_t *n_entries, int64_t ovf_cap,
                                int32_t *ovf_aln, int32_t *ovf_pos, int32_t *ovf_k, int64_t *n_ovf);
+/*   bb_count_kmer_alternatives_wide  the same count for 12 < k <= 16 with a 128-bit key, two words per key in keys_out:
+ *                               [2i] = read k-mer (2 bits a base from bit 0 up, at most 32 bases), [2i+1] = (reference k-mer
+ *                               << 6) | read k-mer length; first_out and counts_out as above.  Longer read k-mers overflow. */
+BB_API int bb_count_kmer_alternatives_wide(int device, int k, int32_t n_aln, const uint8_t *read, const int64_t *read_off,
+                                    const uint8_t *ref, const int64_t *ref_off, const uint32_t *ops, const int32_t *op_read0,
+                                    const int32_t *op_ref0, const int64_t *ops_off, int64_t table_cap, uint64_t *keys_out,
+                                    uint64_t *first_out, uint32_t *counts_out, int64_t *n_entries, int64_t ovf_cap,
+                                    int32_t *ovf_aln, int32_t *ovf_pos, int32_t *ovf_k, int64_t *n_ovf);
 BB_API int bb_count_cigar_qscores(int device, int k, int max_del, int32_t n_aln, const uint8_t *read, const uint8_t *qual,
                            const int64_t *read_off, const uint8_t *ref, const int64_t *ref_off, const uint32_t *ops,
                            const int32_t *op_read0, const int32_t *op_ref0, const int64_t *ops_off, int64_t table_cap,
