@@ -21,6 +21,10 @@ BB_SEG_REF_FWD, BB_SEG_REF_REV, BB_SEG_LITERAL = 0, 1, 2
 BB_N_STAGES = 8
 # bb_rerun_reason: what made a batch run again (bb_last_run_retries)
 BB_RERUN_ROUNDS, BB_RERUN_SLACK, BB_RERUN_LEVELS, BB_RERUN_QUEUES, BB_RERUN_SCRATCH = 1, 2, 4, 8, 16
+# bb_work_slot / bb_node_class: the task counts of bb_last_run_work
+WORK_SLOTS = ('window_lane4', 'window_lane8', 'window_warp', 'leaf_lane', 'leaf_warp', 'root_leaf_lane', 'root_leaf_warp')
+NODE_CLASSES = ('lane8', 'lean1', 'lean2', 'lean4', 'wide')
+BB_MAX_LEVELS = 48
 
 
 class Segment(ctypes.Structure):
@@ -95,6 +99,7 @@ def lib():
         'bb_batch_run': (c.c_int, [vp]),
         'bb_synchronize': (c.c_int, [vp]),
         'bb_last_run_retries': (c.c_int, [vp, P(i32), P(c.c_uint32)]),
+        'bb_last_run_work': (c.c_int, [vp, vp, vp, i32, P(i32)]),
         'bb_host_alloc': (c.c_int, [P(vp), i64]),
         'bb_host_free': (c.c_int, [vp]),
         'bb_last_run_ms': (c.c_int, [vp, P(c.c_float), P(c.c_float)]),
@@ -137,7 +142,7 @@ def lib():
 EXPORTED_SYMBOLS = ['bb_create', 'bb_destroy', 'bb_last_error', 'bb_version', 'bb_upload_reference',
                     'bb_upload_error_model', 'bb_upload_error_model_kmers', 'bb_upload_qscore_model', 'bb_upload_qscore_model_cigars', 'bb_sequence_batch',
                     'bb_fetch_last_batch', 'bb_batch_upload', 'bb_batch_run', 'bb_synchronize', 'bb_last_run_retries',
-                    'bb_host_alloc', 'bb_host_free',
+                    'bb_last_run_work', 'bb_host_alloc', 'bb_host_free',
                     'bb_last_run_ms', 'bb_stage_name', 'bb_launch_count', 'bb_trace_dump', 'bb_get_qscores', 'bb_align_path',
                     'bb_host_align_kmers', 'bb_host_align_path', 'bb_nccl_available', 'bb_comm_unique_id', 'bb_comm_init_rank',
                     'bb_comm_init_all', 'bb_allreduce_bases', 'bb_allreduce_bases_all', 'bb_planner_create', 'bb_planner_destroy',

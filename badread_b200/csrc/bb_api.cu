@@ -38,6 +38,13 @@ struct DevBuf {  // grow-only device allocation
 };
 
 constexpr int BB_MAX_ROUNDS = 15;  // error-loop rounds a run can enqueue (16 counters each, see BB_ROUND_BASE)
+// per-level snapshot of the queue counters (bb_last_run_work): [pipeline][level < BB_MAX_LEVELS][the BBQ_NODE_CLASSES
+// node counts; at level 0 also the two leaf counters right after bb_k_push_roots]
+constexpr int BB_SNAP_WORDS = 8, BB_SNAP_LEAF = BBQ_NODE_CLASSES;
+static_assert(BB_SNAP_LEAF + 2 <= BB_SNAP_WORDS, "snapshot row too short");
+static_assert(BB_NODE_CLASSES == BBQ_NODE_CLASSES && BB_NODE_LANE8 == BBQ_NODE_LANE8 && BB_NODE_LEAN1 == BBQ_NODE_LEAN1 &&
+              BB_NODE_LEAN2 == BBQ_NODE_LEAN2 && BB_NODE_LEAN4 == BBQ_NODE_LEAN4 && BB_NODE_WIDE == BBQ_NODE_WIDE,
+              "bb_node_class must follow the node queues");
 
 const char *kStageNames[BB_N_STAGES] = {"build_fragments", "error_loop", "scan", "join", "final_align", "qscores",
                                         "compact", "total"};
@@ -79,7 +86,10 @@ struct bb_ctx {
     int extra_levels = 0;
     bool lr_worst = false;     // size the split-score scratch for the worst case instead of the expected edit count
     int lr_cap = 0;            // > 0: split-score scratch of a batch starts at this many rows (BADREAD_B200_LR_CAP)
-    struct RunInfo { BBScanOut scan; int counters[256]; int qcount[2][32]; } *h_info = nullptr;  // pinned
+    struct RunInfo {
+        BBScanOut scan; int counters[256]; int qcount[2][32];
+        int levels[2][BB_MAX_LEVELS][BB_SNAP_WORDS];  // queue counters at the start of every level (d_levels)
+    } *h_info = nullptr;  // pinned
     std::vector<BBReadDev> h_res;  // per-read records of the finished run
     bool finished = false;
     bool reran = false;        // w_finish had to run the batch again (copies enqueued before that are stale)
@@ -93,6 +103,7 @@ struct bb_ctx {
     int n_lane_reads = 0, n_long_reads = 0;
     std::vector<int> h_order;
     DevBuf d_kidx, d_frag, d_state, d_seq, d_ops, d_dcnt, d_qual, d_out_seq, d_out_qual, d_counter, d_fpeq, d_speq, d_fallback;
+    DevBuf d_levels;  // int[2][BB_MAX_LEVELS][BB_SNAP_WORDS]: what RunInfo::levels is copied from
     int64_t fpeq_total = 0;
 
     // scratch
@@ -305,7 +316,7 @@ extern "C" int bb_destroy(bb_ctx *ctx) {
                       &ctx->d_qual, &ctx->d_out_seq, &ctx->d_out_qual, &ctx->d_counter, &ctx->s_hist, &ctx->s_hbuf,
                       &ctx->s_lr, &ctx->s_stack, &ctx->s_tbuf, &ctx->s_peq, &ctx->s_ltbuf, &ctx->d_ctime, &ctx->d_chlog, &ctx->d_wres,
                       &ctx->d_wtasks, &ctx->d_wfallback, &ctx->d_active,
-                      &ctx->d_fpeq, &ctx->d_speq, &ctx->d_fallback, &ctx->s_leafhist, &ctx->s_lr_lean, &ctx->s_wckpt, &ctx->s_lanehist, &ctx->d_scan, &ctx->d_red,
+                      &ctx->d_fpeq, &ctx->d_speq, &ctx->d_fallback, &ctx->d_levels, &ctx->s_leafhist, &ctx->s_lr_lean, &ctx->s_wckpt, &ctx->s_lanehist, &ctx->d_scan, &ctx->d_red,
                       &ctx->p_q, &ctx->p_t, &ctx->p_ops, &ctx->p_dcnt, &ctx->p_out, &ctx->p_qual};
     for (auto &qb : ctx->qbuf) {
         for (auto &cl : qb.node) for (auto &d : cl) d.release();
@@ -565,6 +576,7 @@ static int w_prepare(bb_ctx *ctx) {
     BB_CUDA(ctx, ctx->d_kidx.ensure(((size_t)off + 16) * sizeof(int)));
     BB_CUDA(ctx, ctx->d_counter.ensure(BB_N_COUNTERS * sizeof(int)));
     BB_CUDA(ctx, ctx->d_scan.ensure(sizeof(BBScanOut)));
+    BB_CUDA(ctx, ctx->d_levels.ensure(sizeof(bb_ctx::RunInfo::levels)));
     BB_CUDA(ctx, ctx->d_fpeq.ensure(((size_t)ctx->fpeq_total + 4) * sizeof(uint4)));
     BB_CUDA(ctx, ctx->d_ctime.ensure(((size_t)off + 16) * sizeof(unsigned int)));
     BB_CUDA(ctx, ctx->d_chlog.ensure(((size_t)ctx->log_total + 16) * sizeof(uint2)));
@@ -609,7 +621,7 @@ static int w_prepare(bb_ctx *ctx) {
         for (int w = 0; w < 2; w++) BB_CUDA(ctx, qb.leaf[w].ensure((size_t)cap_node * sizeof(BBNode)));
         BB_CUDA(ctx, qb.count.ensure(512 * sizeof(int)));
     }
-    ctx->n_levels = std::max(1, std::min(48, level_bound(ctx->max_len, ctx->slack) + ctx->extra_levels));
+    ctx->n_levels = std::max(1, std::min(BB_MAX_LEVELS, level_bound(ctx->max_len, ctx->slack) + ctx->extra_levels));
     return BB_OK;
 }
 
@@ -756,6 +768,8 @@ static int enqueue_align_tasks(bb_ctx *ctx, const BBBatchDev &B) {
         Q[s].lane8_cols = ctx->lane8_cols;
         BB_CUDA(ctx, cudaMemsetAsync(cnt[s], 0, 512 * sizeof(int), stream[0]));
     }
+    int *snap = ctx->d_levels.as<int>();
+    BB_CUDA(ctx, cudaMemsetAsync(snap, 0, sizeof(bb_ctx::RunInfo::levels), stream[0]));
     bb_k_push_roots<<<(n + 255) / 256, 256, 0, stream[0]>>>(B, Q[0], Q[1], ctx->d_order.as<int>());
     ctx->launches++;
     // pipeline 0 (stream 0): every read whose root band fits the lean / lane kernels; pipeline 1 (stream 1): reads
@@ -774,6 +788,12 @@ static int enqueue_align_tasks(bb_ctx *ctx, const BBBatchDev &B) {
         const int p = (level & 1) | (level > 0 && ctx->lpt_order ? BBQ_BACKWARDS : 0);
         for (int s = 0; s < 2; s++) {
             cudaStream_t st = stream[s];
+            // this level's node counts are final here and cleared when the next level starts: keep them
+            // (bb_last_run_work); the leaf counters at level 0 are the roots' leaves
+            int *row = snap + (s * BB_MAX_LEVELS + level) * BB_SNAP_WORDS;
+            BB_CUDA(ctx, cudaMemcpyAsync(row, cnt[s] + BBQ_COUNT(0, p & 1), BBQ_NODE_CLASSES * sizeof(int), cudaMemcpyDeviceToDevice, st));
+            if (level == 0)
+                BB_CUDA(ctx, cudaMemcpyAsync(row + BB_SNAP_LEAF, cnt[s] + BBQ_LEAF_COUNT, 2 * sizeof(int), cudaMemcpyDeviceToDevice, st));
             BB_CUDA(ctx, cudaMemsetAsync(cnt[s] + BBQ_COUNT(0, (p & 1) ^ 1), 0, BBQ_NODE_CLASSES * sizeof(int), st));
             BB_CUDA(ctx, cudaEventRecord(ctx->ev_level[s], st));
             int n_side = 0;
@@ -825,6 +845,7 @@ static int enqueue_align_tasks(bb_ctx *ctx, const BBBatchDev &B) {
     BB_CUDA(ctx, cudaStreamWaitEvent(stream[0], ctx->ev_join, 0));
     for (int s = 0; s < 2; s++)
         BB_CUDA(ctx, cudaMemcpyAsync(ctx->h_info->qcount[s], cnt[s], 32 * sizeof(int), cudaMemcpyDeviceToHost, stream[0]));
+    BB_CUDA(ctx, cudaMemcpyAsync(ctx->h_info->levels, snap, sizeof(bb_ctx::RunInfo::levels), cudaMemcpyDeviceToHost, stream[0]));
     return BB_OK;
 }
 
@@ -1115,6 +1136,38 @@ extern "C" int bb_last_run_retries(const bb_ctx *ctx, int32_t *n_reruns, uint32_
     }
     if (n_reruns) *n_reruns = total;
     if (reasons) *reasons = bits;
+    return BB_OK;
+}
+
+// Task counts of the last run of every worker (see include/badread_b200.h); read from the counters w_finish fetched.
+extern "C" int bb_last_run_work(const bb_ctx *ctx, int64_t *work, int64_t *level_nodes, int32_t level_cap, int32_t *n_levels) {
+    if (!ctx) return BB_ERR_ARG;
+    if (level_cap < 0 || (level_cap > 0 && !level_nodes)) return set_err(const_cast<bb_ctx *>(ctx), BB_ERR_ARG, "bb_last_run_work: bad arguments");
+    int64_t w[BB_WORK_SLOTS] = {};
+    if (level_nodes) std::fill(level_nodes, level_nodes + (size_t)level_cap * BBQ_NODE_CLASSES, 0);
+    int levels = 0;
+    for (int x = 0; x < ctx->n_split; x++) {
+        const bb_ctx *wk = x == 0 ? ctx : ctx->kids[(size_t)x - 1];
+        if (!wk->finished) return set_err(const_cast<bb_ctx *>(ctx), BB_ERR_STATE, "bb_last_run_work: fetch the batch first");
+        const bb_ctx::RunInfo &info = *wk->h_info;
+        for (int r = 0; r < wk->n_rounds; r++) {  // each kernel passes what it cannot take on to the next
+            const int *c = info.counters + BB_ROUND_BASE(r);
+            w[BB_WORK_WINDOW_LANE4] += c[BBC_NTASKS] - c[BBC_FB1];
+            w[BB_WORK_WINDOW_LANE8] += c[BBC_FB1] - c[BBC_FB2];
+            w[BB_WORK_WINDOW_WARP] += c[BBC_FB2];
+        }
+        for (int s = 0; s < 2; s++) {
+            w[BB_WORK_LEAF_LANE] += info.qcount[s][BBQ_LEAF_COUNT];
+            w[BB_WORK_LEAF_WARP] += info.qcount[s][BBQ_LEAF_COUNT + 1];
+            w[BB_WORK_ROOT_LEAF_LANE] += info.levels[s][0][BB_SNAP_LEAF];
+            w[BB_WORK_ROOT_LEAF_WARP] += info.levels[s][0][BB_SNAP_LEAF + 1];
+            for (int l = 0; l < std::min(level_cap, BB_MAX_LEVELS); l++)
+                for (int c = 0; c < BBQ_NODE_CLASSES; c++) level_nodes[(size_t)l * BBQ_NODE_CLASSES + c] += info.levels[s][l][c];
+        }
+        levels = std::max(levels, wk->n_levels);
+    }
+    if (work) std::memcpy(work, w, sizeof(w));
+    if (n_levels) *n_levels = levels;
     return BB_OK;
 }
 

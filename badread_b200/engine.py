@@ -238,6 +238,21 @@ class Engine(object):
         self._check(self._lib.bb_last_run_retries(self._ctx, ctypes.byref(n), ctypes.byref(reasons)), 'bb_last_run_retries')
         return int(n.value), int(reasons.value)
 
+    def last_run_work(self):
+        """Which alignment kernels the last batch's final run gave work to (bb_last_run_work), summed over the workers:
+        window alignments per kernel ('window_lane4', 'window_lane8', 'window_warp'), Hirschberg leaves per kernel
+        ('leaf_lane', 'leaf_warp', and 'root_leaf_lane' / 'root_leaf_warp' of them that were whole reads), and
+        'levels': for every level the run enqueued, the nodes queued for it per node class, in _lib.NODE_CLASSES
+        order.  Available once the batch has been fetched."""
+        work = np.zeros(len(_lib.WORK_SLOTS), dtype=np.int64)
+        levels = np.zeros((_lib.BB_MAX_LEVELS, len(_lib.NODE_CLASSES)), dtype=np.int64)
+        n = ctypes.c_int32(0)
+        self._check(self._lib.bb_last_run_work(self._ctx, _ptr(work), _ptr(levels), _lib.BB_MAX_LEVELS, ctypes.byref(n)),
+                    'bb_last_run_work')
+        out = {name: int(v) for name, v in zip(_lib.WORK_SLOTS, work)}
+        out['levels'] = [[int(x) for x in row] for row in levels[:n.value]]
+        return out
+
     def launch_count(self):
         return int(self._lib.bb_launch_count(self._ctx))
 

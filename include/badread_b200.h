@@ -158,6 +158,29 @@ enum bb_rerun_reason {
     BB_RERUN_SCRATCH = 16  /* per-warp alignment scratch too small */
 };
 BB_API int bb_last_run_retries(const bb_ctx *ctx, int32_t *n_reruns, uint32_t *reasons);
+/* Diagnostics: which alignment kernels the last run of the last batch gave work to, summed over the workers and both
+ * final-alignment pipelines (the run after any re-runs; complete once the batch has been fetched, BB_ERR_STATE before).
+ *  work[BB_WORK_SLOTS]: window alignments by kernel (the 4-word lane kernel takes every window first and passes the
+ *    ones beyond its limits on to the 8-word lane kernel, which passes its own on to the warp kernel), summed over the
+ *    error-loop rounds; Hirschberg leaves by kernel, all of them and those that were whole roots.
+ *  level_nodes[level_cap][BB_NODE_CLASSES]: Hirschberg nodes queued for each level (0: the roots that are not leaves)
+ *    by node kernel class; levels the run did not reach hold 0.
+ *  *n_levels: Hirschberg levels the run enqueued (at most BB_MAX_LEVELS). */
+enum bb_work_slot {
+    BB_WORK_WINDOW_LANE4 = 0,     /* bb_k_window_lane_hist<4> (bb_k_window_lane<4> with BADREAD_B200_LOWMEM=1) */
+    BB_WORK_WINDOW_LANE8 = 1,     /* bb_k_window_lane_hist<8> / bb_k_window_lane<8> */
+    BB_WORK_WINDOW_WARP = 2,      /* bb_k_window_warp */
+    BB_WORK_LEAF_LANE = 3,        /* bb_k_leaf_lane_hist / bb_k_leaf_lane */
+    BB_WORK_LEAF_WARP = 4,        /* bb_k_leaf_warp */
+    BB_WORK_ROOT_LEAF_LANE = 5,   /* ... of BB_WORK_LEAF_LANE: roots (whole reads) */
+    BB_WORK_ROOT_LEAF_WARP = 6,   /* ... of BB_WORK_LEAF_WARP: roots */
+    BB_WORK_SLOTS = 7
+};
+/* node classes of level_nodes: bb_k_node_lane<8>, bb_k_node_warp<1>, <2>, <4>, and wide nodes (bb_k_node_pair, or
+ * bb_k_node_quad with BADREAD_B200_QUAD=1) */
+enum bb_node_class { BB_NODE_LANE8 = 0, BB_NODE_LEAN1 = 1, BB_NODE_LEAN2 = 2, BB_NODE_LEAN4 = 3, BB_NODE_WIDE = 4, BB_NODE_CLASSES = 5 };
+#define BB_MAX_LEVELS 48
+BB_API int bb_last_run_work(const bb_ctx *ctx, int64_t *work, int64_t *level_nodes, int32_t level_cap, int32_t *n_levels);
 /* CUDA-event time (ms) of the last bb_batch_run on the ctx stream, total and per stage
  * (stage_ms[BB_N_STAGES], see bb_stage_name). Synchronizes. */
 #define BB_N_STAGES 8

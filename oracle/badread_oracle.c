@@ -411,10 +411,52 @@ static uint8_t *reversed(const uint8_t *s, int64_t n) {
     return r;
 }
 
-/* edlib.cpp obtainAlignment / obtainAlignmentHirschberg */
-static void obtain_alignment(const uint8_t *q, int64_t n, const uint8_t *t, int64_t m, int64_t best, opbuf *out) {
+/* Tree of a final alignment (tests only).  After bo_tree_arm(1), this thread's next final alignment - the one
+ * get_qscores makes, or a bo_align_path call - records every obtain_alignment / naive_obtain call with n > 0 and m > 0
+ * in call order, BO_TREE_FIELDS values each: depth, q0, nn, t0, mm, best, is_leaf, target_has_non_acgt.  The window
+ * alignments of the error loop are never recorded.  Thread-local: bo_sequence_batch's workers record their own reads. */
+#define BO_TREE_FIELDS 8
+typedef struct { int64_t *v; int64_t n, cap; const uint8_t *q_base, *t_base; } tree_rec;
+static __thread int t_tree_armed = 0;
+static __thread tree_rec t_tree_buf = {0};   /* the last recorded tree, until bo_tree_take */
+static __thread tree_rec *t_tree = NULL;     /* set while a final alignment records */
+
+static void tree_begin(const uint8_t *q, const uint8_t *t) {
+    if (!t_tree_armed) return;
+    t_tree_armed = 0;
+    free(t_tree_buf.v);
+    memset(&t_tree_buf, 0, sizeof(t_tree_buf));
+    t_tree_buf.q_base = q; t_tree_buf.t_base = t;
+    t_tree = &t_tree_buf;
+}
+static void tree_end(void) { t_tree = NULL; }
+static void tree_add(int depth, const uint8_t *q, int64_t n, const uint8_t *t, int64_t m, int64_t best, int leaf) {
+    tree_rec *r = t_tree;
+    if (!r) return;
+    if (r->n + BO_TREE_FIELDS > r->cap) {
+        r->cap = r->cap ? 2 * r->cap : 64 * BO_TREE_FIELDS;
+        r->v = (int64_t *)realloc(r->v, (size_t)r->cap * sizeof(int64_t));
+    }
+    int non_acgt = 0;
+    for (int64_t j = 0; j < m && !non_acgt; j++) non_acgt = t[j] != 'A' && t[j] != 'C' && t[j] != 'G' && t[j] != 'T';
+    int64_t *e = r->v + r->n;
+    r->n += BO_TREE_FIELDS;
+    e[0] = depth; e[1] = q - r->q_base; e[2] = n; e[3] = t - r->t_base; e[4] = m; e[5] = best; e[6] = leaf; e[7] = non_acgt;
+}
+BO_EXPORT void bo_tree_arm(int on) { t_tree_armed = on; }
+/* Hands the last recorded tree over: returns its number of entries, *out (release with bo_free) their values. */
+BO_EXPORT int64_t bo_tree_take(int64_t **out) {
+    const int64_t n = t_tree_buf.n / BO_TREE_FIELDS;
+    *out = t_tree_buf.v;
+    memset(&t_tree_buf, 0, sizeof(t_tree_buf));
+    return n;
+}
+
+/* edlib.cpp obtainAlignment / obtainAlignmentHirschberg (depth: of this call in the recursion, for the tree) */
+static void obtain_alignment(const uint8_t *q, int64_t n, const uint8_t *t, int64_t m, int64_t best, opbuf *out, int depth) {
     if (n == 0) { op_push(out, 'D', m); return; }
     if (m == 0) { op_push(out, 'I', n); return; }
+    tree_add(depth, q, n, t, m, best, uses_traceback(n, m));
     if (uses_traceback(n, m)) { leaf_traceback(q, n, t, m, best, out); return; }
 
     int64_t left_w = m / 2, right_w = m - left_w;
@@ -442,8 +484,8 @@ static void obtain_alignment(const uint8_t *q, int64_t n, const uint8_t *t, int6
     free(sl); free(sr);
     if (split == -2) { fprintf(stderr, "oracle: Hirschberg found no split\n"); abort(); }
     int64_t ul_h = split + 1;
-    obtain_alignment(q, ul_h, t, left_w, left_score, out);
-    obtain_alignment(q + ul_h, n - ul_h, t + left_w, right_w, right_score, out);
+    obtain_alignment(q, ul_h, t, left_w, left_score, out, depth + 1);
+    obtain_alignment(q + ul_h, n - ul_h, t + left_w, right_w, right_score, out, depth + 1);
 }
 
 /* Full expanded CIGAR of edlib.align(q, t, task='path'); caller frees out->ops. */
@@ -451,7 +493,7 @@ static void align_path(const uint8_t *q, int64_t n, const uint8_t *t, int64_t m,
     int64_t best = nw_distance(q, n, t, m);
     if (dist) *dist = best;
     t_count_blocks = 1;
-    obtain_alignment(q, n, t, m, best, out);
+    obtain_alignment(q, n, t, m, best, out, 0);
     t_count_blocks = 0;
 }
 
@@ -470,9 +512,10 @@ static void naive_matrix(const uint8_t *q, int64_t n, const uint8_t *t, int64_t 
         }
     }
 }
-static void naive_obtain(const uint8_t *q, int64_t n, const uint8_t *t, int64_t m, int64_t best, opbuf *out) {
+static void naive_obtain(const uint8_t *q, int64_t n, const uint8_t *t, int64_t m, int64_t best, opbuf *out, int depth) {
     if (n == 0) { op_push(out, 'D', m); return; }
     if (m == 0) { op_push(out, 'I', n); return; }
+    tree_add(depth, q, n, t, m, best, uses_traceback(n, m));
     int64_t w = m + 1;
     if (uses_traceback(n, m)) {
         int32_t *D = (int32_t *)malloc((size_t)((n + 1) * w) * 4);
@@ -507,15 +550,17 @@ static void naive_obtain(const uint8_t *q, int64_t n, const uint8_t *t, int64_t 
     if (split == -2) { int64_t a = DL[n * (left_w + 1) + left_w]; if (a + right_w == best) { split = n - 1; ls = a; rs = right_w; } }
     free(DL); free(DR);
     if (split == -2) { fprintf(stderr, "oracle: naive Hirschberg found no split\n"); abort(); }
-    naive_obtain(q, split + 1, t, left_w, ls, out);
-    naive_obtain(q + split + 1, n - split - 1, t + left_w, right_w, rs, out);
+    naive_obtain(q, split + 1, t, left_w, ls, out, depth + 1);
+    naive_obtain(q + split + 1, n - split - 1, t + left_w, right_w, rs, out, depth + 1);
 }
 
 /* Python-facing: expanded CIGAR into a malloc'd buffer the caller releases with bo_free. */
 BO_EXPORT int64_t bo_align_path(const uint8_t *q, int64_t n, const uint8_t *t, int64_t m, int naive,
                                 uint8_t **ops_out, int64_t *dist_out) {
     opbuf out = {0};
+    tree_begin(q, t);
     if (n == 0 || m == 0) { /* edlibAlign returns no alignment when either sequence is empty */
+        tree_end();
         *ops_out = NULL; if (dist_out) *dist_out = n > m ? n : m; return -1;
     }
     int64_t best;
@@ -524,10 +569,11 @@ BO_EXPORT int64_t bo_align_path(const uint8_t *q, int64_t n, const uint8_t *t, i
         naive_matrix(q, n, t, m, D);
         best = D[n * (m + 1) + m];
         free(D);
-        naive_obtain(q, n, t, m, best, &out);
+        naive_obtain(q, n, t, m, best, &out, 0);
     } else {
         align_path(q, n, t, m, &out, &best);
     }
+    tree_end();
     if (dist_out) *dist_out = best;
     *ops_out = out.ops;
     return out.n;
@@ -736,7 +782,9 @@ static uint8_t get_qscore(const bo_qm *qm, bo_rng *rng, const uint8_t *cigar, in
 static void get_qscores(const bo_qm *qm, bo_rng *rng, const uint8_t *seq, int64_t seq_len, const uint8_t *frag,
                         int64_t frag_len, uint8_t *qual, int64_t *matches, int64_t *cols) {
     opbuf cg = {0};
+    tree_begin(seq, frag);  /* the final alignment (bo_tree_arm) */
     align_path(seq, seq_len, frag, frag_len, &cg, NULL); /* query = mutated read, target = original */
+    tree_end();
     identity_counts(&cg, matches, cols);
     int64_t *pos2col = (int64_t *)malloc((size_t)seq_len * 8);
     int64_t i = 0;
@@ -902,6 +950,7 @@ typedef struct {
     const bo_em *em; const bo_qm *qm; uint64_t seed; const uint64_t *read_index; const uint8_t *frags;
     const int64_t *frag_off; int32_t n_reads; const double *target_identity; uint8_t **seq_ptrs;
     uint8_t **qual_ptrs; int64_t *out_len, *matches, *cols; int32_t next;
+    int64_t *stats; int64_t **tree_ptrs; int64_t *tree_len;  /* optional (bo_sequence_batch_stats) */
 } batch_job;
 
 static void *batch_worker(void *arg) {
@@ -910,12 +959,38 @@ static void *batch_worker(void *arg) {
         int32_t r = __atomic_fetch_add(&jb->next, 1, __ATOMIC_RELAXED);
         if (r >= jb->n_reads) break;
         bo_rng *rng = bo_rng_create(BO_RNG_PHILOX, jb->seed, jb->read_index[r]);
+        if (jb->tree_ptrs) bo_tree_arm(1);
         bo_sequence_fragment(jb->em, jb->qm, rng, jb->frags + jb->frag_off[r], jb->frag_off[r + 1] - jb->frag_off[r],
                              jb->target_identity[r], 1, &jb->seq_ptrs[r], &jb->qual_ptrs[r], &jb->out_len[r],
-                             &jb->matches[r], &jb->cols[r], NULL);
+                             &jb->matches[r], &jb->cols[r], jb->stats ? jb->stats + 4 * (int64_t)r : NULL);
+        if (jb->tree_ptrs) jb->tree_len[r] = bo_tree_take(&jb->tree_ptrs[r]);
         bo_rng_destroy(rng);
     }
     return NULL;
+}
+
+static int64_t sequence_batch(batch_job *jb, int n_threads) {
+    if (n_threads < 1) n_threads = 1;
+    if (n_threads > 256) n_threads = 256;
+    pthread_t th[256];
+    for (int i = 1; i < n_threads; i++) pthread_create(&th[i], NULL, batch_worker, jb);
+    batch_worker(jb);
+    for (int i = 1; i < n_threads; i++) pthread_join(th[i], NULL);
+    int64_t total = 0;
+    for (int32_t r = 0; r < jb->n_reads; r++) total += jb->out_len[r];
+    return total;
+}
+
+/* bo_sequence_batch that also returns every read's stats[4] (as bo_sequence_fragment's) and the tree of its final
+ * alignment (tree_ptrs[r]: tree_len[r] entries of BO_TREE_FIELDS values, release each with bo_free). */
+BO_EXPORT int64_t bo_sequence_batch_stats(const bo_em *em, const bo_qm *qm, uint64_t seed, const uint64_t *read_index,
+                                          const uint8_t *frags, const int64_t *frag_off, int32_t n_reads,
+                                          const double *target_identity, uint8_t **seq_ptrs, uint8_t **qual_ptrs,
+                                          int64_t *out_len, int64_t *matches, int64_t *cols, int n_threads,
+                                          int64_t *stats, int64_t **tree_ptrs, int64_t *tree_len) {
+    batch_job jb = {em, qm, seed, read_index, frags, frag_off, n_reads, target_identity,
+                    seq_ptrs, qual_ptrs, out_len, matches, cols, 0, stats, tree_ptrs, tree_len};
+    return sequence_batch(&jb, n_threads);
 }
 
 BO_EXPORT int64_t bo_sequence_batch(const bo_em *em, const bo_qm *qm, uint64_t seed, const uint64_t *read_index,
@@ -923,14 +998,6 @@ BO_EXPORT int64_t bo_sequence_batch(const bo_em *em, const bo_qm *qm, uint64_t s
                                     const double *target_identity, uint8_t **seq_ptrs, uint8_t **qual_ptrs,
                                     int64_t *out_len, int64_t *matches, int64_t *cols, int n_threads) {
     batch_job jb = {em, qm, seed, read_index, frags, frag_off, n_reads, target_identity,
-                    seq_ptrs, qual_ptrs, out_len, matches, cols, 0};
-    if (n_threads < 1) n_threads = 1;
-    if (n_threads > 256) n_threads = 256;
-    pthread_t th[256];
-    for (int i = 1; i < n_threads; i++) pthread_create(&th[i], NULL, batch_worker, &jb);
-    batch_worker(&jb);
-    for (int i = 1; i < n_threads; i++) pthread_join(th[i], NULL);
-    int64_t total = 0;
-    for (int32_t r = 0; r < n_reads; r++) total += out_len[r];
-    return total;
+                    seq_ptrs, qual_ptrs, out_len, matches, cols, 0, NULL, NULL, NULL};
+    return sequence_batch(&jb, n_threads);
 }

@@ -72,6 +72,11 @@ def lib():
         L.bo_block_steps.argtypes = []
         L.bo_block_steps.restype = i64
         L.bo_sequence_batch.argtypes = [vp, vp, u64, vp, vp, vp, i32, vp, vp, vp, vp, vp, vp, c.c_int]
+        L.bo_sequence_batch_stats.restype = i64
+        L.bo_sequence_batch_stats.argtypes = [vp, vp, u64, vp, vp, vp, i32, vp, vp, vp, vp, vp, vp, c.c_int, vp, vp, vp]
+        L.bo_tree_arm.argtypes = [c.c_int]
+        L.bo_tree_take.restype = i64
+        L.bo_tree_take.argtypes = [P(vp)]
         _lib = L
     return _lib
 
@@ -84,18 +89,47 @@ def _bytes(s):
     return s.encode('latin-1') if isinstance(s, str) else bytes(s)
 
 
-def align_path(query, target, naive=False):
-    """edlib.align(query, target, task='path') -> (expanded ops string or None, edit distance)."""
+TREE_FIELDS = ('depth', 'q0', 'nn', 't0', 'mm', 'best', 'is_leaf', 'target_has_non_acgt')
+
+
+def _tree_from(ptr, n, L=None):
+    """bo_tree_take's entries as a list of TREE_FIELDS tuples (and the buffer released by library L)."""
+    if not n:
+        return []
+    flat = np.ctypeslib.as_array(ctypes.cast(ptr, ctypes.POINTER(ctypes.c_int64)), shape=(n * len(TREE_FIELDS),))
+    tree = [tuple(int(x) for x in row) for row in flat.reshape(n, len(TREE_FIELDS))]
+    (L or lib()).bo_free(ptr)
+    return tree
+
+
+def _take_tree(L=None):
+    """The tree the last final alignment of this thread recorded in library L (this oracle's by default)."""
+    L = L or lib()
+    ptr = ctypes.c_void_p()
+    n = L.bo_tree_take(ctypes.byref(ptr))
+    return _tree_from(ptr, n, L)
+
+
+def align_path(query, target, naive=False, with_tree=False):
+    """edlib.align(query, target, task='path') -> (expanded ops string or None, edit distance[, tree]).
+
+    with_tree: also the Hirschberg tree of the alignment - every call of obtain_alignment (naive_obtain with
+    naive=True) with both sides non-empty, in call order, as (depth, q0, nn, t0, mm, best, is_leaf,
+    target_has_non_acgt)."""
     L = lib()
     q, t = _bytes(query), _bytes(target)
     out = ctypes.c_void_p()
     dist = ctypes.c_int64(0)
+    if with_tree:
+        L.bo_tree_arm(1)
     n = L.bo_align_path(q, len(q), t, len(t), 1 if naive else 0, ctypes.byref(out), ctypes.byref(dist))
+    tree = _take_tree() if with_tree else None
     if n < 0:
-        return None, dist.value
-    ops = ctypes.string_at(out, n).decode('ascii')
-    L.bo_free(out)
-    return ops, dist.value
+        ops = None
+    else:
+        ops = ctypes.string_at(out, n).decode('ascii')
+        L.bo_free(out)
+    return (ops, dist.value, tree) if with_tree else (ops, dist.value)
 
 
 def set_traceback_limit(v):
@@ -152,7 +186,10 @@ class Oracle(object):
 
     def sequence_fragment(self, fragment, target_identity, seed, read_index=0, mode=RNG_PHILOX, pow_mode=None,
                           with_stats=False):
-        """simulate.sequence_fragment -> (seq, qual, actual_identity[, stats])."""
+        """simulate.sequence_fragment -> (seq, qual, actual_identity[, stats]).
+
+        stats['tree'] is the Hirschberg tree of the final alignment (the untrimmed read against the padded fragment;
+        see align_path's with_tree); the window alignments of the error loop are not in it."""
         L = lib()
         if pow_mode is None:
             pow_mode = 0 if mode == RNG_MT else 1
@@ -161,8 +198,11 @@ class Oracle(object):
         seq, qual = ctypes.c_void_p(), ctypes.c_void_p()
         n, m, c = ctypes.c_int64(0), ctypes.c_int64(0), ctypes.c_int64(0)
         stats = np.zeros(4, dtype=np.int64)
+        if with_stats:
+            L.bo_tree_arm(1)
         L.bo_sequence_fragment(self._em, self._qm, rng, frag, len(frag), target_identity, pow_mode, ctypes.byref(seq),
                                ctypes.byref(qual), ctypes.byref(n), ctypes.byref(m), ctypes.byref(c), _ptr(stats))
+        tree = _take_tree() if with_stats else None
         s = ctypes.string_at(seq, n.value).decode('latin-1')
         q = ctypes.string_at(qual, n.value).decode('latin-1')
         L.bo_free(seq)
@@ -172,7 +212,7 @@ class Oracle(object):
         if with_stats:
             return s, q, ident, {'matches': m.value, 'columns': c.value, 'loop_count': int(stats[0]),
                                  'change_count': int(stats[1]), 'n_alignments': int(stats[2]),
-                                 'untrimmed_len': int(stats[3])}
+                                 'untrimmed_len': int(stats[3]), 'tree': tree}
         return s, q, ident
 
     def get_qscores(self, seq, frag, seed, read_index=0, mode=RNG_PHILOX):
@@ -193,9 +233,11 @@ class Oracle(object):
         L.bo_add_errors_to_kmer(self._em, rng._h, kb, _ptr(out), _ptr(off))
         return [bytes(out[off[j]:off[j + 1]]).decode('latin-1') for j in range(self.k)]
 
-    def sequence_batch(self, fragments, target_identities, seed, read_indices, n_threads=1):
+    def sequence_batch(self, fragments, target_identities, seed, read_indices, n_threads=1, with_stats=False):
         """Philox-mode batch over independent reads with `n_threads` host threads (the timed CPU baseline).
-        Returns (list of (seq, qual, matches, columns), total_bases)."""
+        Returns (list of (seq, qual, matches, columns), total_bases).  with_stats: every read's tuple gains a fifth
+        item, the stats dict of sequence_fragment(..., with_stats=True) without 'matches' / 'columns' (the tree
+        included)."""
         L = lib()
         n = len(fragments)
         frs = [_bytes(f) for f in fragments]
@@ -209,15 +251,28 @@ class Oracle(object):
         out_len = np.zeros(n, dtype=np.int64)
         matches = np.zeros(n, dtype=np.int64)
         cols = np.zeros(n, dtype=np.int64)
-        total = L.bo_sequence_batch(self._em, self._qm, ctypes.c_uint64(seed), _ptr(ri), _ptr(blob), _ptr(off), n,
-                                    _ptr(ti), seq_ptrs, qual_ptrs, _ptr(out_len), _ptr(matches), _ptr(cols), n_threads)
+        if with_stats:
+            stats = np.zeros((max(n, 1), 4), dtype=np.int64)
+            tree_ptrs = (ctypes.c_void_p * n)()
+            tree_len = np.zeros(n, dtype=np.int64)
+            total = L.bo_sequence_batch_stats(self._em, self._qm, ctypes.c_uint64(seed), _ptr(ri), _ptr(blob), _ptr(off),
+                                              n, _ptr(ti), seq_ptrs, qual_ptrs, _ptr(out_len), _ptr(matches), _ptr(cols),
+                                              n_threads, _ptr(stats), tree_ptrs, _ptr(tree_len))
+        else:
+            total = L.bo_sequence_batch(self._em, self._qm, ctypes.c_uint64(seed), _ptr(ri), _ptr(blob), _ptr(off), n,
+                                        _ptr(ti), seq_ptrs, qual_ptrs, _ptr(out_len), _ptr(matches), _ptr(cols), n_threads)
         out = []
         for r in range(n):
             s = ctypes.string_at(seq_ptrs[r], int(out_len[r])).decode('latin-1')
             q = ctypes.string_at(qual_ptrs[r], int(out_len[r])).decode('latin-1')
             L.bo_free(seq_ptrs[r])
             L.bo_free(qual_ptrs[r])
-            out.append((s, q, int(matches[r]), int(cols[r])))
+            if with_stats:
+                st = {'loop_count': int(stats[r, 0]), 'change_count': int(stats[r, 1]), 'n_alignments': int(stats[r, 2]),
+                      'untrimmed_len': int(stats[r, 3]), 'tree': _tree_from(tree_ptrs[r], int(tree_len[r]))}
+                out.append((s, q, int(matches[r]), int(cols[r]), st))
+            else:
+                out.append((s, q, int(matches[r]), int(cols[r])))
         return out, int(total)
 
 

@@ -51,6 +51,9 @@ def lib():
         L.bo_sequence_fragment_kmers.restype = c.c_int
         L.bo_sequence_fragment_kmers.argtypes = [vp, vp, vp, vp, i64, dbl, c.c_int, P(vp), P(vp), P(i64), P(i64), P(i64),
                                                  vp]
+        L.bo_tree_arm.argtypes = [c.c_int]
+        L.bo_tree_take.restype = i64
+        L.bo_tree_take.argtypes = [P(vp)]
         _lib = L
     return _lib
 
@@ -95,9 +98,12 @@ class OracleKmers(object):
         seq, qual = ctypes.c_void_p(), ctypes.c_void_p()
         n, m, c = ctypes.c_int64(0), ctypes.c_int64(0), ctypes.c_int64(0)
         stats = np.zeros(4, dtype=np.int64)
+        if with_stats:
+            L.bo_tree_arm(1)
         L.bo_sequence_fragment_kmers(self._em, self._qm, rng, frag, len(frag), target_identity, pow_mode,
                                      ctypes.byref(seq), ctypes.byref(qual), ctypes.byref(n), ctypes.byref(m),
                                      ctypes.byref(c), _ptr(stats))
+        tree = O._take_tree(L) if with_stats else None
         s = ctypes.string_at(seq, n.value).decode('latin-1')
         q = ctypes.string_at(qual, n.value).decode('latin-1')
         L.bo_free(seq)
@@ -107,7 +113,7 @@ class OracleKmers(object):
         if with_stats:
             return s, q, ident, {'matches': m.value, 'columns': c.value, 'loop_count': int(stats[0]),
                                  'change_count': int(stats[1]), 'n_alignments': int(stats[2]),
-                                 'untrimmed_len': int(stats[3])}
+                                 'untrimmed_len': int(stats[3]), 'tree': tree}
         return s, q, ident
 
 
