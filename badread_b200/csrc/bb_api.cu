@@ -5,10 +5,10 @@
 #include <unistd.h>
 
 #include <algorithm>
-#include <atomic>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <numeric>
 #include <string>
 #include <thread>
@@ -19,21 +19,23 @@
 
 namespace {
 
-struct DevBuf {  // grow-only device allocation
+struct DevBuf {  // grow-only device allocation, freed with its owner
     void *p = nullptr;
     size_t cap = 0;
-    bool borrowed = false;  // p belongs to another context (the workers of a context share its reference and tables)
-    void borrow(const DevBuf &o) { release(); p = o.p; cap = o.cap; borrowed = true; }
+    DevBuf() = default;
+    DevBuf(const DevBuf &) = delete;
+    DevBuf &operator=(const DevBuf &) = delete;  // (so a Worker or a context cannot be copied either)
+    DevBuf(DevBuf &&o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+    ~DevBuf() { release(); }
     cudaError_t ensure(size_t bytes) {
-        if (bytes <= cap && !borrowed) return cudaSuccess;
-        if (borrowed) { p = nullptr; cap = 0; borrowed = false; }
-        if (p) { cudaFree(p); p = nullptr; cap = 0; }
+        if (bytes <= cap) return cudaSuccess;
+        release();
         size_t want = bytes + bytes / 8 + 256;
         cudaError_t e = cudaMalloc(&p, want);
         if (e == cudaSuccess) cap = want;
         return e;
     }
-    void release() { if (p && !borrowed) cudaFree(p); p = nullptr; cap = 0; borrowed = false; }
+    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
     template <typename T> T *as() const { return reinterpret_cast<T *>(p); }
 };
 
@@ -42,124 +44,192 @@ constexpr int BB_MAX_ROUNDS = 15;  // error-loop rounds a run can enqueue (16 co
 // node counts; at level 0 also the two leaf counters right after bb_k_push_roots]
 constexpr int BB_SNAP_WORDS = 8, BB_SNAP_LEAF = BBQ_NODE_CLASSES;
 static_assert(BB_SNAP_LEAF + 2 <= BB_SNAP_WORDS, "snapshot row too short");
-static_assert(BB_NODE_CLASSES == BBQ_NODE_CLASSES && BB_NODE_LANE8 == BBQ_NODE_LANE8 && BB_NODE_LEAN1 == BBQ_NODE_LEAN1 &&
-              BB_NODE_LEAN2 == BBQ_NODE_LEAN2 && BB_NODE_LEAN4 == BBQ_NODE_LEAN4 && BB_NODE_WIDE == BBQ_NODE_WIDE,
+static_assert(int(BB_NODE_CLASSES) == int(BBQ_NODE_CLASSES) && int(BB_NODE_LANE8) == int(BBQ_NODE_LANE8) &&
+              int(BB_NODE_LEAN1) == int(BBQ_NODE_LEAN1) && int(BB_NODE_LEAN2) == int(BBQ_NODE_LEAN2) &&
+              int(BB_NODE_LEAN4) == int(BBQ_NODE_LEAN4) && int(BB_NODE_WIDE) == int(BBQ_NODE_WIDE),
               "bb_node_class must follow the node queues");
+
+// Queue counters of an alignment pipeline: one block of kQueueCounts ints, the BBQ_* counts first, then from
+// kCursorBase one work cursor per node / leaf launch (5 per level at most, 2 for the leaves).
+constexpr int kQueueCounts = 512, kCursorBase = 16;
+static_assert(BBQ_OVERFLOW < kCursorBase && kCursorBase + 5 * BB_MAX_LEVELS + 2 <= kQueueCounts, "queue counter block");
+
+// The single-warp node kernels (4, 2 and 1 words per lane) of both pipelines are resident at once: each launch owns
+// a fixed range of warp slots in pool_lean, sized for its grid cap of kLeanCtasPerSm CTAs per SM.
+enum { LEAN4, LEAN2, LEAN1 };
+constexpr int kLeanCtasPerSm[3] = {4, 6, 6};
+constexpr int kLeanCtasPerSmBoth = 2 * (kLeanCtasPerSm[LEAN4] + kLeanCtasPerSm[LEAN2] + kLeanCtasPerSm[LEAN1]);
 
 const char *kStageNames[BB_N_STAGES] = {"build_fragments", "error_loop", "scan", "join", "final_align", "qscores",
                                         "compact", "total"};
+
+enum GridKnob { G_MUTATE, G_WIN4, G_WIN8, G_WARP1, G_WARP2, G_WARP4, G_LANE8, G_LEAF, kGridKnobs };
+const char *const kGridNames[kGridKnobs] = {"MUTATE", "WIN4", "WIN8", "WARP1", "WARP2", "WARP4", "LANE8", "LEAF"};
+
+// The BADREAD_B200_* environment variables, read once by bb_create (see README).
+struct Knobs {
+    bool trace = false;        // TRACE: an event after every launch / host step of a run (bb_trace_dump)
+    int n_workers = 2;         // SUBBATCHES
+    bool head_priority = true; // HEAD_PRIORITY: worker 0 on high-priority streams
+    bool head_worker = true;   // HEAD_WORKER: worker 0 = the longest reads only (see bb_batch_upload)
+    int grid_div = 0;          // GRID_DIV: > 0 replaces the share of the SMs the workers of a split batch ask for
+    int grid[kGridKnobs] = {}; // GRID_<name>: > 0 replaces the kernel's CTAs per SM
+    int lane8_cols = 4096;     // routing limit of the lane node kernel
+    int pair_ctas = 1;         // CTAs per SM of the warp-pair node kernel
+    bool lpt_order = true;     // node queues below the roots walked from the end (longest nodes first)
+    int ring_t = 4;            // columns per traceback tick of the 4-word window aligner (2, 4 or 8)
+    bool lowmem = false;       // window / leaf aligners with checkpoints + shared-memory tiles instead of global history
+    bool use_quad = false;     // wide nodes by 8-warp CTAs (bb_k_node_quad) instead of warp pairs
+    // starting values of the limits w_finish grows when a batch outgrows them (the results do not depend on them);
+    // lr_cap > 0: the split-score scratch of a batch starts at this many rows
+    int n_rounds = 3, extra_levels = 0, lr_cap = 0;
+    double slack = 1.25;
+};
+
+Knobs read_knobs() {
+    Knobs k;
+    auto env = [](const std::string &name) { return std::getenv(("BADREAD_B200_" + name).c_str()); };
+    if (const char *e = env("TRACE")) k.trace = (e[0] == '1');
+    if (const char *e = env("SUBBATCHES")) k.n_workers = std::max(1, std::min(8, std::atoi(e)));
+    if (const char *e = env("HEAD_PRIORITY")) k.head_priority = (e[0] != '0');
+    if (const char *e = env("HEAD_WORKER")) k.head_worker = (e[0] != '0');
+    if (const char *e = env("GRID_DIV")) k.grid_div = std::atoi(e);
+    for (int g = 0; g < kGridKnobs; g++) if (const char *e = env(std::string("GRID_") + kGridNames[g])) k.grid[g] = std::atoi(e);
+    if (const char *e = env("LANE8_COLS")) k.lane8_cols = std::atoi(e);
+    if (const char *e = env("PAIR_CTAS")) k.pair_ctas = (e[0] == '2') ? 2 : 1;
+    if (const char *e = env("LPT")) k.lpt_order = (e[0] != '0');
+    if (const char *e = env("RING_T")) k.ring_t = (e[0] == '8') ? 8 : (e[0] == '2') ? 2 : 4;
+    if (const char *e = env("LOWMEM")) k.lowmem = (e[0] != '0');
+    if (const char *e = env("QUAD")) k.use_quad = (e[0] != '0');
+    if (const char *e = env("ROUNDS")) k.n_rounds = std::max(1, std::min(BB_MAX_ROUNDS, std::atoi(e)));
+    if (const char *e = env("SLACK")) { const double v = std::atof(e); if (v > 0.0) k.slack = v; }
+    if (const char *e = env("EXTRA_LEVELS")) k.extra_levels = std::atoi(e);
+    if (const char *e = env("LR_CAP")) k.lr_cap = std::max(0, std::atoi(e));
+    return k;
+}
+
+// One kernel chain of a context: its streams, the part of the batch it was dealt, and the buffers, scratch and queues
+// its kernels run on.  The reference, the models and the knobs are the context's.
+struct Worker {
+    bb_ctx *ctx;
+    cudaStream_t stream = nullptr, stream2 = nullptr;
+    cudaStream_t side[2][3] = {};   // per alignment pipeline: the streams of the node classes that run next to the main one
+    cudaEvent_t ev_side[2][3] = {}, ev_level[2] = {};
+    cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_scan = nullptr;
+    cudaEvent_t ev[BB_N_STAGES + 1] = {};
+    std::string err;  // batch uploads run on one host thread per worker
+    int64_t launches = 0;
+
+    // batch
+    int n_reads = 0;
+    bool uploaded = false, ran = false, finished = false;
+    bool is_head = false;      // this worker holds the head batch of the current upload
+    std::vector<BBReadDev> h_reads;
+    std::vector<int32_t> h_inlen;
+    std::vector<double> h_target;
+    int64_t frag_total = 0;
+    int64_t seq_cap = 0, out_cap = 0, speq_cap = 0;  // capacities of the per-batch buffers (from the fragment lengths)
+    int64_t log_total = 0, wres_total = 0, fpeq_total = 0;
+    int max_len = 0;
+    // sizing knobs a retry raises (bb_k_scan / the node kernels flag what did not fit; see w_finish)
+    double slack;              // joined reads may be this much longer than their fragments in total
+    int n_rounds;              // mutate -> windows -> replay rounds enqueued without asking the device in between
+    int n_levels = 0;          // Hirschberg levels enqueued (from the longest fragment)
+    int extra_levels;
+    bool lr_worst = false;     // size the split-score scratch for the worst case instead of the expected edit count
+    struct RunInfo {
+        BBScanOut scan; int counters[256]; int qcount[2][32];
+        int levels[2][BB_MAX_LEVELS][BB_SNAP_WORDS];  // queue counters at the start of every level (d_levels)
+    } *h_info = nullptr;  // pinned
+    std::vector<BBReadDev> h_res;  // per-read records of the finished run
+    bool reran = false;        // w_finish had to run the batch again (copies enqueued before that are stale)
+    int n_reruns = 0;          // runs of the current batch after the first (bb_last_run_retries)
+    uint32_t rerun_reasons = 0;  // BB_RERUN_* bits of what did not fit
+    DevBuf d_read_index, d_seg_off, d_segs, d_lit, d_target, d_order, d_reads;
+    DevBuf d_kidx, d_frag, d_state, d_seq, d_ops, d_dcnt, d_qual, d_out_seq, d_out_qual, d_counter, d_fpeq, d_speq, d_scan;
+    DevBuf d_levels;  // int[2][BB_MAX_LEVELS][BB_SNAP_WORDS]: what RunInfo::levels is copied from
+    DevBuf d_ctime, d_chlog, d_wres, d_wtasks, d_wfallback;
+
+    // Where the kernels of a run find their share of the queues and scratch (set by w_prepare)
+    struct Layout {
+        int cap_node = 0;          // entries of every node and leaf queue
+        int lane_ctas = 0;         // 64-thread CTAs of the lane leaf kernel of one pipeline (its grid cap)
+        size_t hist_per_pipe = 0;  // elements of s_lanehist (s_leafhist with lowmem) that one pipeline's leaf kernel owns
+        int64_t fb_len = 0;        // entries of each of the two window fall-back lists in d_wfallback
+        int lean_base[2][3] = {};  // first pool_lean slot of each pipeline's LEAN4 / LEAN2 / LEAN1 node kernel
+    } L;
+
+    // scratch
+    BBScratchPool pool{}, pool_lean{};  // pool_lean: split-score arrays of the single-warp node kernels (bands < 2048 rows)
+    DevBuf s_hist, s_hbuf, s_lr, s_stack, s_tbuf, s_peq, s_ltbuf, s_leafhist, s_lr_lean, s_wckpt, s_lanehist;
+    DevBuf p_q, p_t, p_ops, p_dcnt, p_out, p_qual;  // single-pair entry points (bb_align_path / bb_get_qscores): kept between calls
+    struct QueueBufs { DevBuf node[BBQ_NODE_CLASSES][2], leaf[2], count; } qbuf[2];  // [0] normal, [1] wide-root reads
+
+    // launch trace (BADREAD_B200_TRACE=1): an event after every launch / host step of a run, dumped by bb_trace_dump
+    struct Mark { const char *name; int stream; cudaEvent_t ev; };
+    std::vector<Mark> marks;
+    std::vector<cudaEvent_t> mark_pool;
+    size_t mark_used = 0;
+
+    Worker(bb_ctx *c, const Knobs &k) : ctx(c), slack(k.slack), n_rounds(k.n_rounds), extra_levels(k.extra_levels) {}
+    ~Worker() {
+        for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
+        for (cudaEvent_t e : {ev_fork, ev_join, ev_scan, ev_level[0], ev_level[1]}) if (e) cudaEventDestroy(e);
+        for (auto &row : ev_side) for (cudaEvent_t e : row) if (e) cudaEventDestroy(e);
+        for (cudaStream_t s : {stream, stream2}) if (s) cudaStreamDestroy(s);
+        for (auto &row : side) for (cudaStream_t s : row) if (s) cudaStreamDestroy(s);
+        for (cudaEvent_t e : mark_pool) cudaEventDestroy(e);
+        if (h_info) cudaFreeHost(h_info);
+    }
+};
 
 }  // namespace
 
 struct bb_ctx {
     int device = 0;
     int sm_count = 0;
+    int n_warps = 0;  // warp slots of a worker's pool (4 CTAs of BB_WARPS_PER_CTA warps per SM)
     uint64_t seed = 0;
-    cudaStream_t stream = nullptr, stream2 = nullptr;
-    cudaStream_t side[2][3] = {};   // per alignment pipeline: the streams of the node classes that run next to the main one
-    cudaEvent_t ev_side[2][3] = {}, ev_level[2] = {};
-    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     std::string err;
-    int64_t launches = 0;
+    Knobs knobs;
 
-    // reference + models
+    // reference + models, shared by the workers
     DevBuf ref; int64_t ref_len = 0;
     bool have_em = false, have_qm = false;
     BBErrorModelDev em{}; DevBuf em_k2r, em_rowoff, em_cum, em_flags, em_slots, em_pool, em_rowinfo;
     BBEmHashDev em_hash{}; DevBuf em_hentries;  // k-mer index as a hash table (bb_upload_error_model_kmers)
     BBQScoreModelDev qm{}; DevBuf qm_hkeys, qm_hvals, qm_lkeys, qm_lpool, qm_rowoff, qm_scores, qm_cum;
 
-    // batch
-    int n_reads = 0;
-    bool uploaded = false, ran = false;
-    std::vector<BBReadDev> h_reads;
-    std::vector<int32_t> h_inlen;
-    std::vector<double> h_target;
-    int64_t frag_total = 0, out_total = 0;
-    int64_t seq_cap = 0, out_cap = 0, speq_cap = 0;  // capacities of the per-batch buffers (from the fragment lengths)
-    int64_t log_total = 0, wres_total = 0;
-    int max_len = 0;
-    // sizing knobs a retry raises (bb_k_scan / the node kernels flag what did not fit; see w_finish)
-    double slack = 1.25;       // joined reads may be this much longer than their fragments in total
-    int n_rounds = 3;          // mutate -> windows -> replay rounds enqueued without asking the device in between
-    int n_levels = 0;          // Hirschberg levels enqueued (from the longest fragment)
-    int extra_levels = 0;
-    bool lr_worst = false;     // size the split-score scratch for the worst case instead of the expected edit count
-    int lr_cap = 0;            // > 0: split-score scratch of a batch starts at this many rows (BADREAD_B200_LR_CAP)
-    struct RunInfo {
-        BBScanOut scan; int counters[256]; int qcount[2][32];
-        int levels[2][BB_MAX_LEVELS][BB_SNAP_WORDS];  // queue counters at the start of every level (d_levels)
-    } *h_info = nullptr;  // pinned
-    std::vector<BBReadDev> h_res;  // per-read records of the finished run
-    bool finished = false;
-    bool reran = false;        // w_finish had to run the batch again (copies enqueued before that are stale)
-    int n_reruns = 0;          // runs of the current batch after the first (bb_last_run_retries)
-    uint32_t rerun_reasons = 0;  // BB_RERUN_* bits of what did not fit
-    DevBuf d_scan;
-    void *nccl_comm = nullptr;   // ncclComm_t of this context's device (bb_comm_init_rank / bb_comm_init_all)
-    DevBuf d_red;                // two int64: send, receive of bb_allreduce_bases
-    cudaEvent_t ev_scan = nullptr;
-    DevBuf d_read_index, d_seg_off, d_segs, d_lit, d_target, d_order, d_reads;
-    int n_lane_reads = 0, n_long_reads = 0;
-    std::vector<int> h_order;
-    DevBuf d_kidx, d_frag, d_state, d_seq, d_ops, d_dcnt, d_qual, d_out_seq, d_out_qual, d_counter, d_fpeq, d_speq, d_fallback;
-    DevBuf d_levels;  // int[2][BB_MAX_LEVELS][BB_SNAP_WORDS]: what RunInfo::levels is copied from
-    int64_t fpeq_total = 0;
-
-    // scratch
-    int n_warps = 0;
-    BBScratchPool pool{}, pool_lean{};  // pool_lean: split-score arrays of the single-warp node kernels (bands < 2048 rows)
-    DevBuf s_hist, s_hbuf, s_lr, s_stack, s_tbuf, s_peq, s_ltbuf, s_leafhist, s_lr_lean, s_wckpt, s_lanehist;
-    DevBuf d_ctime, d_chlog, d_wres, d_wtasks, d_wfallback, d_active;
-    DevBuf p_q, p_t, p_ops, p_dcnt, p_out, p_qual;  // single-pair entry points (bb_align_path / bb_get_qscores): kept between calls
-    int lane8_cols = 4096;  // routing limit of the lane node kernel (tuning knob)
-    int pair_ctas = 1;   // CTAs per SM of the warp-pair node kernel (tuning knob)
-    bool head_worker = true;  // worker 0 = the longest reads only (see bb_batch_upload)
-    bool is_head = false;     // this worker holds the head batch of the current upload
-    bool lpt_order = true;    // node queues below the roots walked from the end (longest nodes first)
-    int ring_t = 4;           // columns per traceback tick of the 4-word window aligner (2, 4 or 8)
-    bool lowmem = false;      // window / leaf aligners with checkpoints + shared-memory tiles instead of global history
-    bool use_quad = false;    // wide nodes by 8-warp CTAs (bb_k_node_quad) instead of warp pairs
-    int grid_div_env = 0;
-    int grid_div = 1;         // persistent grids are launched at 1/grid_div of their full size (the workers of a split batch share the SMs)
-    struct QueueBufs { DevBuf node[BBQ_NODE_CLASSES][2], leaf[2], count; } qbuf[2];  // [0] normal, [1] wide-root reads
-
-
-    cudaEvent_t ev[BB_N_STAGES + 1] = {};
-    float stage_ms[BB_N_STAGES] = {};
-
-    // sub-batches: a context made by bb_create owns n_kids further worker contexts on the same device; a batch is
-    // dealt out over the workers (this context is worker 0) and their kernel chains run side by side on their
-    // own streams, so that one worker's tails and host round trips are covered by the others' kernels
-    std::vector<bb_ctx *> kids;
-    int n_split = 1;                          // workers the uploaded batch is spread over (1: this context alone)
+    // Sub-batches: a batch is dealt out over the workers and their kernel chains run side by side on their own
+    // streams, so that one worker's tails and host round trips are covered by the others' kernels.  Worker 0 also
+    // runs the uploads and the single-pair entry points.
+    std::vector<std::unique_ptr<Worker>> workers;
+    int n_split = 1;                          // workers the uploaded batch is spread over
     std::vector<std::vector<int32_t>> part;   // part[w][i] = batch position of worker w's i-th read
-    std::vector<int64_t> part_base;           // offset of worker w's block in the fetched seq / qual buffers
     cudaEvent_t ev_t0 = nullptr, ev_t1 = nullptr;
 
-    // launch trace (BADREAD_B200_TRACE=1): an event after every launch / host step of a run, dumped by bb_trace_dump
-    bool trace = false;
-    struct Mark { const char *name; int stream; cudaEvent_t ev; };
-    std::vector<Mark> marks;
-    std::vector<cudaEvent_t> mark_pool;
-    size_t mark_used = 0;
+    void *nccl_comm = nullptr;   // ncclComm_t of this context's device (bb_comm_init_rank / bb_comm_init_all)
+    DevBuf d_red;                // two int64: send, receive of bb_allreduce_bases
+
+    Worker &w0() { return *workers[0]; }
+    ~bb_ctx() { for (cudaEvent_t e : {ev_t0, ev_t1}) if (e) cudaEventDestroy(e); }
 };
 
 // Records "the work enqueued on `st` up to here is done" under `name` (tracing only).
-static void mark(bb_ctx *ctx, cudaStream_t st, const char *name) {
-    if (!ctx->trace) return;
-    if (ctx->mark_used == ctx->mark_pool.size()) {
+static void mark(Worker &w, cudaStream_t st, const char *name) {
+    if (!w.ctx->knobs.trace) return;
+    if (w.mark_used == w.mark_pool.size()) {
         cudaEvent_t e;
         if (cudaEventCreate(&e) != cudaSuccess) return;
-        ctx->mark_pool.push_back(e);
+        w.mark_pool.push_back(e);
     }
-    cudaEvent_t e = ctx->mark_pool[ctx->mark_used++];
+    cudaEvent_t e = w.mark_pool[w.mark_used++];
     cudaEventRecord(e, st);
-    int id = st == ctx->stream ? 0 : st == ctx->stream2 ? 1 : -1;
+    int id = st == w.stream ? 0 : st == w.stream2 ? 1 : -1;
     for (int p = 0; p < 2 && id < 0; p++)
         for (int x = 0; x < 3; x++)
-            if (st == ctx->side[p][x]) id = 2 + 4 * p + x;
-    ctx->marks.push_back(bb_ctx::Mark{name, id < 0 ? 0 : id, e});
+            if (st == w.side[p][x]) id = 2 + 4 * p + x;
+    w.marks.push_back(Worker::Mark{name, id < 0 ? 0 : id, e});
 }
 
 static thread_local std::string g_create_error;
@@ -174,6 +244,7 @@ struct ConnectionsDefault {
 } g_connections_default;
 }  // namespace
 
+// (ctx) is a bb_ctx or a Worker: whichever reports the error
 #define BB_CUDA(ctx, call)                                                                                   \
     do {                                                                                                     \
         cudaError_t e_ = (call);                                                                             \
@@ -183,9 +254,20 @@ struct ConnectionsDefault {
         }                                                                                                    \
     } while (0)
 
-static int set_err(bb_ctx *ctx, int code, const std::string &msg) {
-    if (ctx) ctx->err = msg;
+template <typename O>
+static int set_err(O *o, int code, const std::string &msg) {
+    if (o) o->err = msg;
     return code;
+}
+
+// Calls f(worker, w) for the workers of the current split in order; the first failure's code and message become the context's.
+template <typename F>
+static int each_worker(bb_ctx *ctx, F &&f) {
+    for (int w = 0; w < ctx->n_split; w++) {
+        Worker &wk = *ctx->workers[(size_t)w];
+        if (const int rc = f(wk, w)) return set_err(ctx, rc, wk.err);
+    }
+    return BB_OK;
 }
 
 extern "C" const char *bb_version(void) { return "badread_b200 0.1.0 (sm_90a)"; }
@@ -198,12 +280,33 @@ extern "C" const char *bb_stage_name(int stage) {
 
 extern "C" int64_t bb_launch_count(const bb_ctx *ctx) {
     if (!ctx) return 0;
-    int64_t total = ctx->launches;
-    for (const bb_ctx *kid : ctx->kids) total += kid->launches;
+    int64_t total = 0;
+    for (const auto &w : ctx->workers) total += w->launches;
     return total;
 }
 
-static int create_worker(bb_ctx **out, int device, uint64_t seed, bool high_priority = false) {
+static int add_worker(bb_ctx *ctx, bool high_priority) {
+    ctx->workers.push_back(std::make_unique<Worker>(ctx, ctx->knobs));
+    Worker &w = *ctx->workers.back();
+    int prio_lo = 0, prio_hi = 0;
+    cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
+    const int prio = high_priority ? prio_hi : prio_lo;
+    cudaError_t e = cudaStreamCreateWithPriority(&w.stream, cudaStreamNonBlocking, prio);
+    if (e != cudaSuccess) { g_create_error = cudaGetErrorString(e); return BB_ERR_CUDA; }
+    cudaStreamCreateWithPriority(&w.stream2, cudaStreamNonBlocking, prio);
+    for (auto &row : w.side) for (cudaStream_t &s : row) cudaStreamCreateWithPriority(&s, cudaStreamNonBlocking, prio);
+    for (cudaEvent_t &e : w.ev) cudaEventCreate(&e);
+    for (cudaEvent_t *e : {&w.ev_fork, &w.ev_join, &w.ev_scan, &w.ev_level[0], &w.ev_level[1]}) cudaEventCreateWithFlags(e, cudaEventDisableTiming);
+    for (auto &row : w.ev_side) for (cudaEvent_t &e : row) cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
+    if (cudaHostAlloc((void **)&w.h_info, sizeof(Worker::RunInfo), cudaHostAllocPortable) == cudaSuccess) return BB_OK;
+    w.h_info = nullptr;
+    g_create_error = "cudaHostAlloc failed";
+    return BB_ERR_CUDA;
+}
+
+static void (*nccl_destroy)(void *) = nullptr;  // set once NCCL is loaded (bb_comm_init_*)
+
+extern "C" int bb_create(bb_ctx **out, int device, uint64_t seed) {
     if (!out) return BB_ERR_ARG;
     *out = nullptr;
     int n_dev = 0;
@@ -216,35 +319,16 @@ static int create_worker(bb_ctx **out, int device, uint64_t seed, bool high_prio
     if (device < 0 || device >= n_dev) { g_create_error = "invalid device ordinal"; return BB_ERR_ARG; }
     e = cudaSetDevice(device);
     if (e != cudaSuccess) { g_create_error = cudaGetErrorString(e); return BB_ERR_CUDA; }
-    bb_ctx *ctx = new bb_ctx();
+    std::unique_ptr<bb_ctx> ctx(new bb_ctx());
     ctx->device = device;
     ctx->seed = seed;
+    ctx->knobs = read_knobs();
     cudaDeviceProp prop;
     e = cudaGetDeviceProperties(&prop, device);
-    if (e != cudaSuccess) { g_create_error = cudaGetErrorString(e); delete ctx; return BB_ERR_CUDA; }
+    if (e != cudaSuccess) { g_create_error = cudaGetErrorString(e); return BB_ERR_CUDA; }
     ctx->sm_count = prop.multiProcessorCount;
-    // worker 0 carries the longest reads of a split batch (bb_batch_upload): their dependent chain of stages bounds the
-    // step from below, so its kernels go first whenever the block scheduler has a choice
-    int prio_lo = 0, prio_hi = 0;
-    cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
-    const int prio = high_priority ? prio_hi : prio_lo;
-    e = cudaStreamCreateWithPriority(&ctx->stream, cudaStreamNonBlocking, prio);
-    if (e != cudaSuccess) { g_create_error = cudaGetErrorString(e); delete ctx; return BB_ERR_CUDA; }
-    for (auto &ev : ctx->ev) cudaEventCreate(&ev);
-    cudaStreamCreateWithPriority(&ctx->stream2, cudaStreamNonBlocking, prio);
-    cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming);
-    cudaEventCreateWithFlags(&ctx->ev_join, cudaEventDisableTiming);
-    cudaEventCreateWithFlags(&ctx->ev_scan, cudaEventDisableTiming);
-    for (int p = 0; p < 2; p++) {
-        cudaEventCreateWithFlags(&ctx->ev_level[p], cudaEventDisableTiming);
-        for (int x = 0; x < 3; x++) {
-            cudaStreamCreateWithPriority(&ctx->side[p][x], cudaStreamNonBlocking, prio);
-            cudaEventCreateWithFlags(&ctx->ev_side[p][x], cudaEventDisableTiming);
-        }
-    }
-    if (cudaHostAlloc((void **)&ctx->h_info, sizeof(bb_ctx::RunInfo), cudaHostAllocPortable) != cudaSuccess) {
-        g_create_error = "cudaHostAlloc failed"; delete ctx; return BB_ERR_CUDA;
-    }
+    // persistent warps: 4 CTAs of 4 warps per SM for the warp-per-read kernels
+    ctx->n_warps = ctx->sm_count * 4 * BB_WARPS_PER_CTA;
     // misc.REV_COMP_DICT (misc.py:56-61); anything else complements to 'N' (misc.py:64-68)
     uint8_t comp[256];
     std::memset(comp, 'N', sizeof(comp));
@@ -252,125 +336,61 @@ static int create_worker(bb_ctx **out, int device, uint64_t seed, bool high_prio
     const char *to = "TACGtacgYRSWMKVBHDNyrswmkvbhdn.-?";
     for (int i = 0; from[i]; i++) comp[(uint8_t)from[i]] = (uint8_t)to[i];
     e = cudaMemcpyToSymbol(bb_c_comp, comp, 256);
-    if (e != cudaSuccess) { g_create_error = cudaGetErrorString(e); delete ctx; return BB_ERR_CUDA; }
-    e = bbl_node_pair_init();
+    if (e == cudaSuccess) e = bbl_node_pair_init();
     if (e == cudaSuccess) e = bbl_node_quad_init();
     if (e == cudaSuccess) e = bbl_window_lane_init();
     if (e == cudaSuccess) e = bbl_leaf_lane_init();
-    if (e != cudaSuccess) { g_create_error = cudaGetErrorString(e); delete ctx; return BB_ERR_CUDA; }
-    // persistent warps: 4 CTAs of 4 warps per SM for the warp-per-read kernels
-    ctx->n_warps = ctx->sm_count * 4 * BB_WARPS_PER_CTA;
-    if (const char *e = std::getenv("BADREAD_B200_TRACE")) ctx->trace = (e[0] == '1');
-    if (const char *e = std::getenv("BADREAD_B200_LANE8_COLS")) ctx->lane8_cols = std::atoi(e);
-    if (const char *e = std::getenv("BADREAD_B200_PAIR_CTAS")) ctx->pair_ctas = (e[0] == '2') ? 2 : 1;
-    if (const char *e = std::getenv("BADREAD_B200_HEAD_WORKER")) ctx->head_worker = (e[0] != '0');
-    if (const char *e = std::getenv("BADREAD_B200_GRID_DIV")) ctx->grid_div_env = std::atoi(e);
-    if (const char *e = std::getenv("BADREAD_B200_QUAD")) ctx->use_quad = (e[0] != '0');
-    if (const char *e = std::getenv("BADREAD_B200_LOWMEM")) ctx->lowmem = (e[0] != '0');
-    if (const char *e = std::getenv("BADREAD_B200_LPT")) ctx->lpt_order = (e[0] != '0');
-    if (const char *e = std::getenv("BADREAD_B200_RING_T")) ctx->ring_t = (e[0] == '8') ? 8 : (e[0] == '2') ? 2 : 4;
-    // starting values of the limits w_finish grows when a batch outgrows them (the results do not depend on them)
-    if (const char *e = std::getenv("BADREAD_B200_ROUNDS")) ctx->n_rounds = std::max(1, std::min(BB_MAX_ROUNDS, std::atoi(e)));
-    if (const char *e = std::getenv("BADREAD_B200_SLACK")) { const double v = std::atof(e); if (v > 0.0) ctx->slack = v; }
-    if (const char *e = std::getenv("BADREAD_B200_EXTRA_LEVELS")) ctx->extra_levels = std::atoi(e);
-    if (const char *e = std::getenv("BADREAD_B200_LR_CAP")) ctx->lr_cap = std::max(0, std::atoi(e));
-    *out = ctx;
-    return BB_OK;
-}
-
-extern "C" int bb_destroy(bb_ctx *ctx);
-static void (*nccl_destroy)(void *) = nullptr;  // set once NCCL is loaded (bb_comm_init_*)
-
-extern "C" int bb_create(bb_ctx **out, int device, uint64_t seed) {
-    bool prio = true;
-    if (const char *e = std::getenv("BADREAD_B200_HEAD_PRIORITY")) prio = (e[0] != '0');
-    int rc = create_worker(out, device, seed, prio);
-    if (rc) return rc;
-    bb_ctx *ctx = *out;
+    if (e != cudaSuccess) { g_create_error = cudaGetErrorString(e); return BB_ERR_CUDA; }
     // 2 workers on H100 (132 SMs, 80 GB): as fast as 3 and 12 % faster than 4 on config 1, and their scratch (lane
-    // histories sized by the SM count) leaves room for a second context on the same GPU (~39 GB peak against 66 with 4)
-    int n_workers = 2;
-    if (const char *e = std::getenv("BADREAD_B200_SUBBATCHES")) n_workers = std::max(1, std::min(8, std::atoi(e)));
-    for (int w = 1; w < n_workers; w++) {
-        bb_ctx *kid = nullptr;
-        if ((rc = create_worker(&kid, device, seed))) { bb_destroy(ctx); *out = nullptr; return rc; }
-        ctx->kids.push_back(kid);
-    }
+    // histories sized by the SM count) leaves room for a second context on the same GPU (~39 GB peak against 66 with 4).
+    // Worker 0 carries the longest reads of a split batch (bb_batch_upload): their dependent chain of stages bounds the
+    // step from below, so its kernels go first whenever the block scheduler has a choice.
+    for (int w = 0; w < ctx->knobs.n_workers; w++)
+        if (const int rc = add_worker(ctx.get(), w == 0 && ctx->knobs.head_priority)) return rc;
     cudaEventCreate(&ctx->ev_t0);
     cudaEventCreate(&ctx->ev_t1);
+    *out = ctx.release();
     return BB_OK;
 }
 
 extern "C" int bb_destroy(bb_ctx *ctx) {
     if (!ctx) return BB_OK;
-    for (bb_ctx *kid : ctx->kids) bb_destroy(kid);
-    ctx->kids.clear();
-    cudaSetDevice(ctx->device);
-    cudaStreamSynchronize(ctx->stream);
-    if (ctx->ev_t0) cudaEventDestroy(ctx->ev_t0);
-    if (ctx->ev_t1) cudaEventDestroy(ctx->ev_t1);
-    DevBuf *bufs[] = {&ctx->ref, &ctx->em_k2r, &ctx->em_hentries, &ctx->em_rowoff, &ctx->em_cum, &ctx->em_flags, &ctx->em_slots,
-                      &ctx->em_pool, &ctx->em_rowinfo, &ctx->qm_hkeys, &ctx->qm_hvals, &ctx->qm_lkeys, &ctx->qm_lpool, &ctx->qm_rowoff, &ctx->qm_scores, &ctx->qm_cum,
-                      &ctx->d_read_index, &ctx->d_seg_off, &ctx->d_segs, &ctx->d_lit, &ctx->d_target, &ctx->d_order,
-                      &ctx->d_reads, &ctx->d_kidx, &ctx->d_frag, &ctx->d_state, &ctx->d_seq, &ctx->d_ops, &ctx->d_dcnt,
-                      &ctx->d_qual, &ctx->d_out_seq, &ctx->d_out_qual, &ctx->d_counter, &ctx->s_hist, &ctx->s_hbuf,
-                      &ctx->s_lr, &ctx->s_stack, &ctx->s_tbuf, &ctx->s_peq, &ctx->s_ltbuf, &ctx->d_ctime, &ctx->d_chlog, &ctx->d_wres,
-                      &ctx->d_wtasks, &ctx->d_wfallback, &ctx->d_active,
-                      &ctx->d_fpeq, &ctx->d_speq, &ctx->d_fallback, &ctx->d_levels, &ctx->s_leafhist, &ctx->s_lr_lean, &ctx->s_wckpt, &ctx->s_lanehist, &ctx->d_scan, &ctx->d_red,
-                      &ctx->p_q, &ctx->p_t, &ctx->p_ops, &ctx->p_dcnt, &ctx->p_out, &ctx->p_qual};
-    for (auto &qb : ctx->qbuf) {
-        for (auto &cl : qb.node) for (auto &d : cl) d.release();
-        qb.leaf[0].release(); qb.leaf[1].release(); qb.count.release();
-    }
-    for (DevBuf *b : bufs) b->release();
-    for (auto &ev : ctx->ev) if (ev) cudaEventDestroy(ev);
-    cudaStreamDestroy(ctx->stream);
-    if (ctx->stream2) cudaStreamDestroy(ctx->stream2);
-    if (ctx->ev_fork) cudaEventDestroy(ctx->ev_fork);
-    if (ctx->ev_join) cudaEventDestroy(ctx->ev_join);
-    if (ctx->ev_scan) cudaEventDestroy(ctx->ev_scan);
-    for (int p = 0; p < 2; p++) {
-        if (ctx->ev_level[p]) cudaEventDestroy(ctx->ev_level[p]);
-        for (int x = 0; x < 3; x++) {
-            if (ctx->side[p][x]) cudaStreamDestroy(ctx->side[p][x]);
-            if (ctx->ev_side[p][x]) cudaEventDestroy(ctx->ev_side[p][x]);
-        }
-    }
-    if (ctx->h_info) cudaFreeHost(ctx->h_info);
+    cudaSetDevice(ctx->device);  // the frees below act on the current device
+    for (const auto &w : ctx->workers) cudaStreamSynchronize(w->stream);
     if (ctx->nccl_comm && nccl_destroy) nccl_destroy(ctx->nccl_comm);
-    for (cudaEvent_t e : ctx->mark_pool) cudaEventDestroy(e);
     delete ctx;
     return BB_OK;
 }
 
-template <typename T>
-static int upload(bb_ctx *ctx, DevBuf &buf, const T *src, size_t count) {
-    BB_CUDA(ctx, buf.ensure(std::max<size_t>(count, 1) * sizeof(T)));
-    if (count) BB_CUDA(ctx, cudaMemcpyAsync(buf.p, src, count * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
+template <typename O, typename T>
+static int upload(O *o, cudaStream_t st, DevBuf &buf, const T *src, size_t count) {
+    BB_CUDA(o, buf.ensure(std::max<size_t>(count, 1) * sizeof(T)));
+    if (count) BB_CUDA(o, cudaMemcpyAsync(buf.p, src, count * sizeof(T), cudaMemcpyHostToDevice, st));
     return BB_OK;
 }
 
 extern "C" int bb_upload_reference(bb_ctx *ctx, const uint8_t *bases, int64_t n_bases) {
     if (!ctx || n_bases < 0 || (n_bases && !bases)) return set_err(ctx, BB_ERR_ARG, "bb_upload_reference: bad arguments");
     BB_CUDA(ctx, cudaSetDevice(ctx->device));
-    int rc = upload(ctx, ctx->ref, bases, (size_t)n_bases);
+    const cudaStream_t st = ctx->w0().stream;
+    int rc = upload(ctx, st, ctx->ref, bases, (size_t)n_bases);
     if (rc) return rc;
-    BB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    BB_CUDA(ctx, cudaStreamSynchronize(st));
     ctx->ref_len = n_bases;
-    for (bb_ctx *kid : ctx->kids) { kid->ref.borrow(ctx->ref); kid->ref_len = n_bases; }  // one copy per GPU
     return BB_OK;
 }
 
 // The per-entry tables of a model (everything but the k-mer index) and the per-row summaries derived from them.
 static int upload_em_rows(bb_ctx *ctx, int k, int32_t n_rows, const int32_t *row_off, const double *cum,
                           const uint8_t *flags, const uint32_t *slots, const uint8_t *pool, int64_t pool_len) {
+    const cudaStream_t st = ctx->w0().stream;
     const int64_t ne = row_off[n_rows];
     int rc;
-    if ((rc = upload(ctx, ctx->em_rowoff, row_off, (size_t)n_rows + 1))) return rc;
-    if ((rc = upload(ctx, ctx->em_cum, cum, (size_t)ne))) return rc;
-    if ((rc = upload(ctx, ctx->em_flags, flags, (size_t)ne))) return rc;
-    if ((rc = upload(ctx, ctx->em_slots, slots, (size_t)ne * k))) return rc;
-    if ((rc = upload(ctx, ctx->em_pool, pool, (size_t)pool_len))) return rc;
+    if ((rc = upload(ctx, st, ctx->em_rowoff, row_off, (size_t)n_rows + 1))) return rc;
+    if ((rc = upload(ctx, st, ctx->em_cum, cum, (size_t)ne))) return rc;
+    if ((rc = upload(ctx, st, ctx->em_flags, flags, (size_t)ne))) return rc;
+    if ((rc = upload(ctx, st, ctx->em_slots, slots, (size_t)ne * k))) return rc;
+    if ((rc = upload(ctx, st, ctx->em_pool, pool, (size_t)pool_len))) return rc;
     std::vector<BBRowInfo> info((size_t)n_rows);
     for (int32_t r = 0; r < n_rows; r++) {
         const int32_t e0 = row_off[r], ne = row_off[r + 1] - e0;
@@ -379,21 +399,13 @@ static int upload_em_rows(bb_ctx *ctx, int k, int32_t n_rows, const int32_t *row
         ri.cum_last = cum[e0 + ne - 1]; ri.cum0 = cum[e0]; ri.e0 = e0; ri.ne = ne;
         ri.first_is_identity = flags[e0] == 1 ? 1 : 0; ri.pad = 0;
     }
-    if ((rc = upload(ctx, ctx->em_rowinfo, info.data(), info.size()))) return rc;
-    BB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // `info` is about to go out of scope
+    if ((rc = upload(ctx, st, ctx->em_rowinfo, info.data(), info.size()))) return rc;
+    BB_CUDA(ctx, cudaStreamSynchronize(st));  // `info` is about to go out of scope
     ctx->em.row_off = ctx->em_rowoff.as<int32_t>();
     ctx->em.cum = ctx->em_cum.as<double>(); ctx->em.flags = ctx->em_flags.as<uint8_t>();
     ctx->em.slots = ctx->em_slots.as<uint32_t>(); ctx->em.pool = ctx->em_pool.as<uint8_t>();
     ctx->em.rowinfo = ctx->em_rowinfo.as<BBRowInfo>();
     return BB_OK;
-}
-
-static void share_em(bb_ctx *ctx) {
-    ctx->have_em = true;
-    ctx->uploaded = false;
-    for (bb_ctx *kid : ctx->kids) {  // shared tables
-        kid->em = ctx->em; kid->em_hash = ctx->em_hash; kid->have_em = true; kid->uploaded = false;
-    }
 }
 
 extern "C" int bb_upload_error_model(bb_ctx *ctx, int k, int type, const int32_t *kmer_to_row, int64_t n_index,
@@ -409,12 +421,13 @@ extern "C" int bb_upload_error_model(bb_ctx *ctx, int k, int type, const int32_t
         if (!kmer_to_row || !row_off || !cum || !flags || !slots || n_rows <= 0 || n_index != (1ll << (2 * k)))
             return set_err(ctx, BB_ERR_ARG, "error model: missing tables");
         int rc;
-        if ((rc = upload(ctx, ctx->em_k2r, kmer_to_row, (size_t)n_index))) return rc;
+        if ((rc = upload(ctx, ctx->w0().stream, ctx->em_k2r, kmer_to_row, (size_t)n_index))) return rc;
         if ((rc = upload_em_rows(ctx, k, n_rows, row_off, cum, flags, slots, pool, pool_len))) return rc;
         ctx->em.kmer_to_row = ctx->em_k2r.as<int32_t>();
     }
-    BB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    share_em(ctx);
+    BB_CUDA(ctx, cudaStreamSynchronize(ctx->w0().stream));
+    ctx->have_em = true;
+    for (const auto &w : ctx->workers) w->uploaded = false;  // the fragment layout of a batch depends on k
     return BB_OK;
 }
 
@@ -432,11 +445,12 @@ extern "C" int bb_upload_error_model_kmers(bb_ctx *ctx, int k, int32_t n_rows, c
     ctx->em_hash = BBEmHashDev{};
     ctx->have_em = false;
     int rc;
-    if ((rc = upload(ctx, ctx->em_hentries, t.entries.data(), t.entries.size()))) return rc;
+    if ((rc = upload(ctx, ctx->w0().stream, ctx->em_hentries, t.entries.data(), t.entries.size()))) return rc;
     if ((rc = upload_em_rows(ctx, k, n_rows, row_off, cum, flags, slots, pool, pool_len))) return rc;  // (synchronizes)
     ctx->em.k = k; ctx->em.type = 1;
     ctx->em_hash.entries = ctx->em_hentries.as<unsigned long long>(); ctx->em_hash.bits = t.bits;
-    share_em(ctx);
+    ctx->have_em = true;
+    for (const auto &w : ctx->workers) w->uploaded = false;  // the fragment layout of a batch depends on k
     return BB_OK;
 }
 
@@ -450,16 +464,17 @@ extern "C" int bb_upload_qscore_model_cigars(bb_ctx *ctx, int kmer_size, int32_t
     BBQScoreTables t;
     std::string err;
     if (!bb_build_qscore_tables(n_keys, key_chars, key_off, t, err)) return set_err(ctx, BB_ERR_ARG, err);
+    const cudaStream_t st = ctx->w0().stream;
     const int64_t ne = row_off[n_keys];
     int rc;
-    if ((rc = upload(ctx, ctx->qm_hkeys, t.hkeys.data(), t.hkeys.size()))) return rc;
-    if ((rc = upload(ctx, ctx->qm_hvals, t.hvals.data(), t.hvals.size()))) return rc;
-    if ((rc = upload(ctx, ctx->qm_lkeys, t.lkeys.data(), t.lkeys.size()))) return rc;
-    if ((rc = upload(ctx, ctx->qm_lpool, t.lpool.data(), t.lpool.size()))) return rc;
-    if ((rc = upload(ctx, ctx->qm_rowoff, row_off, (size_t)n_keys + 1))) return rc;
-    if ((rc = upload(ctx, ctx->qm_scores, scores, (size_t)ne))) return rc;
-    if ((rc = upload(ctx, ctx->qm_cum, cum, (size_t)ne))) return rc;
-    BB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if ((rc = upload(ctx, st, ctx->qm_hkeys, t.hkeys.data(), t.hkeys.size()))) return rc;
+    if ((rc = upload(ctx, st, ctx->qm_hvals, t.hvals.data(), t.hvals.size()))) return rc;
+    if ((rc = upload(ctx, st, ctx->qm_lkeys, t.lkeys.data(), t.lkeys.size()))) return rc;
+    if ((rc = upload(ctx, st, ctx->qm_lpool, t.lpool.data(), t.lpool.size()))) return rc;
+    if ((rc = upload(ctx, st, ctx->qm_rowoff, row_off, (size_t)n_keys + 1))) return rc;
+    if ((rc = upload(ctx, st, ctx->qm_scores, scores, (size_t)ne))) return rc;
+    if ((rc = upload(ctx, st, ctx->qm_cum, cum, (size_t)ne))) return rc;
+    BB_CUDA(ctx, cudaStreamSynchronize(st));
     ctx->qm.kmer_size = kmer_size; ctx->qm.hbits = t.hbits;
     ctx->qm.hkeys = ctx->qm_hkeys.as<uint64_t>(); ctx->qm.hvals = ctx->qm_hvals.as<int32_t>();
     ctx->qm.row_off = ctx->qm_rowoff.as<int32_t>(); ctx->qm.scores = ctx->qm_scores.as<uint8_t>();
@@ -467,7 +482,6 @@ extern "C" int bb_upload_qscore_model_cigars(bb_ctx *ctx, int kmer_size, int32_t
     ctx->qm.long_max_len = t.long_max_len; ctx->qm.lbits = t.lbits;
     ctx->qm.lkeys = ctx->qm_lkeys.as<BBQLongKey>(); ctx->qm.lpool = ctx->qm_lpool.as<uint64_t>();
     ctx->have_qm = true;
-    for (bb_ctx *kid : ctx->kids) { kid->qm = ctx->qm; kid->have_qm = true; }  // shared tables
     return BB_OK;
 }
 
@@ -483,8 +497,8 @@ extern "C" int bb_upload_qscore_model(bb_ctx *ctx, int kmer_size, int32_t n_keys
 
 // Scratch shared by the warp-per-read kernels. hist is sized for the largest traceback edlib's 1 MiB rule
 // admits (ceil(n/64)*m < 52429 -> < 104858 32-row blocks); tbuf holds a joined 1000-slot window.
-static int ensure_scratch(bb_ctx *ctx, int hbuf_need, int lr_need, int len_need, int lr_floor = 4096) {
-    const int n_warps = ctx->n_warps;
+static int ensure_scratch(Worker &w, int hbuf_need, int lr_need, int len_need, int lr_floor = 4096) {
+    const int n_warps = w.ctx->n_warps;
     const int hist_cap = 106496;
     const int tbuf_stride = 1000 * 255 + 1024;
     const int stack_cap = 64;
@@ -494,55 +508,55 @@ static int ensure_scratch(bb_ctx *ctx, int hbuf_need, int lr_need, int len_need,
     lr_cap = (lr_cap + 255) & ~255;
     int peq_cap = bb_peq_words(len_need) + 8;
     peq_cap = (peq_cap + 63) & ~63;
-    if (ctx->pool.peq_cap >= peq_cap) peq_cap = ctx->pool.peq_cap;
-    if (ctx->pool.hbuf_cap >= hbuf_cap) hbuf_cap = ctx->pool.hbuf_cap;
-    if (ctx->pool.lr_cap >= lr_cap) lr_cap = ctx->pool.lr_cap;
-    BB_CUDA(ctx, ctx->s_hist.ensure((size_t)n_warps * hist_cap * sizeof(uint2)));
-    BB_CUDA(ctx, ctx->s_tbuf.ensure((size_t)n_warps * tbuf_stride));
-    BB_CUDA(ctx, ctx->s_stack.ensure((size_t)n_warps * stack_cap * 5 * sizeof(int)));
-    BB_CUDA(ctx, ctx->s_hbuf.ensure((size_t)n_warps * hbuf_cap));
-    BB_CUDA(ctx, ctx->s_lr.ensure((size_t)n_warps * lr_cap * 2 * sizeof(int)));
-    BB_CUDA(ctx, ctx->s_peq.ensure((size_t)n_warps * peq_cap * sizeof(uint4)));
-    BBScratchPool &p = ctx->pool;
-    p.hist = ctx->s_hist.as<uint2>(); p.hist_stride = hist_cap; p.hist_cap = hist_cap;
-    p.hbuf = ctx->s_hbuf.as<int8_t>(); p.hbuf_stride = hbuf_cap; p.hbuf_cap = hbuf_cap;
-    p.lr = ctx->s_lr.as<int>(); p.lr_stride = 2ll * lr_cap; p.lr_cap = lr_cap;
-    p.stack = ctx->s_stack.as<int>(); p.stack_cap = stack_cap;
-    p.tbuf = ctx->s_tbuf.as<uint8_t>(); p.tbuf_stride = tbuf_stride;
-    p.peq = ctx->s_peq.as<uint4>(); p.peq_stride = peq_cap; p.peq_cap = peq_cap;
-    // the single-warp node kernels (2 pipelines x 3 widths, all resident at once) only touch the split-score arrays
+    if (w.pool.peq_cap >= peq_cap) peq_cap = w.pool.peq_cap;
+    if (w.pool.hbuf_cap >= hbuf_cap) hbuf_cap = w.pool.hbuf_cap;
+    if (w.pool.lr_cap >= lr_cap) lr_cap = w.pool.lr_cap;
+    BB_CUDA(&w, w.s_hist.ensure((size_t)n_warps * hist_cap * sizeof(uint2)));
+    BB_CUDA(&w, w.s_tbuf.ensure((size_t)n_warps * tbuf_stride));
+    BB_CUDA(&w, w.s_stack.ensure((size_t)n_warps * stack_cap * 5 * sizeof(int)));
+    BB_CUDA(&w, w.s_hbuf.ensure((size_t)n_warps * hbuf_cap));
+    BB_CUDA(&w, w.s_lr.ensure((size_t)n_warps * lr_cap * 2 * sizeof(int)));
+    BB_CUDA(&w, w.s_peq.ensure((size_t)n_warps * peq_cap * sizeof(uint4)));
+    BBScratchPool &p = w.pool;
+    p.hist = w.s_hist.as<uint2>(); p.hist_stride = hist_cap; p.hist_cap = hist_cap;
+    p.hbuf = w.s_hbuf.as<int8_t>(); p.hbuf_stride = hbuf_cap; p.hbuf_cap = hbuf_cap;
+    p.lr = w.s_lr.as<int>(); p.lr_stride = 2ll * lr_cap; p.lr_cap = lr_cap;
+    p.stack = w.s_stack.as<int>(); p.stack_cap = stack_cap;
+    p.tbuf = w.s_tbuf.as<uint8_t>(); p.tbuf_stride = tbuf_stride;
+    p.peq = w.s_peq.as<uint4>(); p.peq_stride = peq_cap; p.peq_cap = peq_cap;
+    // the single-warp node kernels only touch the split-score arrays
     constexpr int lean_cap = 2048;  // > a + b + 1 of the widest lean class (bb_pick_L<4>(a, b, 16) > 0: a + b < 1920)
-    const size_t lean_warps = 2 * (size_t)ctx->sm_count * (4 + 6 + 6) * BB_WARPS_PER_CTA;  // room for the grid knobs' maxima
-    BB_CUDA(ctx, ctx->s_lr_lean.ensure(lean_warps * lean_cap * 2 * sizeof(int)));
-    ctx->pool_lean = p;
-    ctx->pool_lean.lr = ctx->s_lr_lean.as<int>(); ctx->pool_lean.lr_stride = 2ll * lean_cap; ctx->pool_lean.lr_cap = lean_cap;
+    const size_t lean_warps = (size_t)w.ctx->sm_count * kLeanCtasPerSmBoth * BB_WARPS_PER_CTA;
+    BB_CUDA(&w, w.s_lr_lean.ensure(lean_warps * lean_cap * 2 * sizeof(int)));
+    w.pool_lean = p;
+    w.pool_lean.lr = w.s_lr_lean.as<int>(); w.pool_lean.lr_stride = 2ll * lean_cap; w.pool_lean.lr_cap = lean_cap;
     return BB_OK;
 }
 
-static BBBatchDev batch_dev(bb_ctx *ctx) {
+static BBBatchDev batch_dev(const Worker &w) {
     BBBatchDev B{};
-    B.n_reads = ctx->n_reads;
-    B.read_index = ctx->d_read_index.as<unsigned long long>();
-    B.seg_off = ctx->d_seg_off.as<int>();
-    B.segs = ctx->d_segs.as<bb_segment>();
-    B.lit = ctx->d_lit.as<uint8_t>();
-    B.target = ctx->d_target.as<double>();
-    B.order = ctx->d_order.as<int>();
-    B.reads = ctx->d_reads.as<BBReadDev>();
-    B.frag = ctx->d_frag.as<uint8_t>();
-    B.state = ctx->d_state.as<uint32_t>();
-    B.kidx = ctx->d_kidx.as<int>();
-    B.seq = ctx->d_seq.as<uint8_t>();
-    B.ops = ctx->d_ops.as<uint8_t>();
-    B.dcnt = ctx->d_dcnt.as<unsigned int>();
-    B.qual = ctx->d_qual.as<uint8_t>();
-    B.out_seq = ctx->d_out_seq.as<uint8_t>();
-    B.out_qual = ctx->d_out_qual.as<uint8_t>();
-    B.fpeq = ctx->d_fpeq.as<uint4>();
-    B.speq = ctx->d_speq.as<uint4>();
-    B.ctime = ctx->d_ctime.as<unsigned int>();
-    B.chlog = ctx->d_chlog.as<uint2>();
-    B.wres = ctx->d_wres.as<int2>();
+    B.n_reads = w.n_reads;
+    B.read_index = w.d_read_index.as<unsigned long long>();
+    B.seg_off = w.d_seg_off.as<int>();
+    B.segs = w.d_segs.as<bb_segment>();
+    B.lit = w.d_lit.as<uint8_t>();
+    B.target = w.d_target.as<double>();
+    B.order = w.d_order.as<int>();
+    B.reads = w.d_reads.as<BBReadDev>();
+    B.frag = w.d_frag.as<uint8_t>();
+    B.state = w.d_state.as<uint32_t>();
+    B.kidx = w.d_kidx.as<int>();
+    B.seq = w.d_seq.as<uint8_t>();
+    B.ops = w.d_ops.as<uint8_t>();
+    B.dcnt = w.d_dcnt.as<unsigned int>();
+    B.qual = w.d_qual.as<uint8_t>();
+    B.out_seq = w.d_out_seq.as<uint8_t>();
+    B.out_qual = w.d_out_qual.as<uint8_t>();
+    B.fpeq = w.d_fpeq.as<uint4>();
+    B.speq = w.d_speq.as<uint4>();
+    B.ctime = w.d_ctime.as<unsigned int>();
+    B.chlog = w.d_chlog.as<uint2>();
+    B.wres = w.d_wres.as<int2>();
     return B;
 }
 
@@ -564,83 +578,89 @@ static int level_bound(int max_len, double slack) {
 // Every allocation a run needs, sized from the fragment lengths: a run is pure enqueueing, nothing on the host
 // depends on a value the device computes.  What turns out too small is flagged by the kernels and w_finish grows
 // the knobs (slack, n_rounds, levels, lr_worst) and runs the batch again.
-static int w_prepare(bb_ctx *ctx) {
-    BB_CUDA(ctx, cudaSetDevice(ctx->device));
-    const int n = ctx->n_reads;
-    const int64_t off = ctx->frag_total;
-    ctx->seq_cap = (int64_t)((double)off * ctx->slack) + 16ll * n + 65536;
-    ctx->out_cap = ctx->seq_cap;
-    ctx->speq_cap = ctx->seq_cap / 32 + (2ll * BB_PEQ_PAD + 2) * n + 64;
-    BB_CUDA(ctx, ctx->d_frag.ensure((size_t)off + 16));
-    BB_CUDA(ctx, ctx->d_state.ensure(((size_t)off + 16) * sizeof(uint32_t)));
-    BB_CUDA(ctx, ctx->d_kidx.ensure(((size_t)off + 16) * sizeof(int)));
-    BB_CUDA(ctx, ctx->d_counter.ensure(BB_N_COUNTERS * sizeof(int)));
-    BB_CUDA(ctx, ctx->d_scan.ensure(sizeof(BBScanOut)));
-    BB_CUDA(ctx, ctx->d_levels.ensure(sizeof(bb_ctx::RunInfo::levels)));
-    BB_CUDA(ctx, ctx->d_fpeq.ensure(((size_t)ctx->fpeq_total + 4) * sizeof(uint4)));
-    BB_CUDA(ctx, ctx->d_ctime.ensure(((size_t)off + 16) * sizeof(unsigned int)));
-    BB_CUDA(ctx, ctx->d_chlog.ensure(((size_t)ctx->log_total + 16) * sizeof(uint2)));
-    BB_CUDA(ctx, ctx->d_wres.ensure(((size_t)ctx->wres_total + 16) * sizeof(int2)));
-    BB_CUDA(ctx, ctx->d_wtasks.ensure(((size_t)ctx->wres_total + 16) * sizeof(BBWinTask)));
-    BB_CUDA(ctx, ctx->d_wfallback.ensure((2 * (size_t)ctx->wres_total + 16) * sizeof(BBWinTask)));
-    BB_CUDA(ctx, ctx->d_seq.ensure((size_t)ctx->seq_cap + 16));
-    BB_CUDA(ctx, ctx->d_ops.ensure((size_t)ctx->seq_cap + 16));
-    BB_CUDA(ctx, ctx->d_dcnt.ensure(((size_t)ctx->seq_cap + 16) * sizeof(unsigned int)));
-    BB_CUDA(ctx, ctx->d_qual.ensure((size_t)ctx->seq_cap + 16));
-    BB_CUDA(ctx, ctx->d_speq.ensure(((size_t)ctx->speq_cap + 4) * sizeof(uint4)));
-    BB_CUDA(ctx, ctx->d_out_seq.ensure((size_t)ctx->out_cap + 16));
-    BB_CUDA(ctx, ctx->d_out_qual.ensure((size_t)ctx->out_cap + 16));
-    const int lane_ctas = ctx->sm_count * 4;  // 64-thread CTAs of the lane kernels
-    {   // lane pools of the window aligner and the leaf aligner (the two alignment pipelines each own half)
-        const size_t lanes = (size_t)lane_ctas * 64;
-        if (ctx->lowmem) BB_CUDA(ctx, ctx->s_leafhist.ensure(2 * lanes * BB_LEAF_MAX_TILES * BB_LEAF_CKPT_WORDS * sizeof(uint32_t)));
-        else BB_CUDA(ctx, ctx->s_lanehist.ensure(2 * lanes * BB_LEAF_LANE_COLS * BB_LEAF_LW * sizeof(uint2)));  // per-column history
-        BB_CUDA(ctx, ctx->s_ltbuf.ensure(2 * lanes * BB_WIN_MAX_COLS));  // the 4-word window kernel runs up to 1.5x the lanes
-        // window aligners: a checkpoint (2 LW + 2 words) per 16 columns per lane instead of a per-column history
-        if (ctx->lowmem) BB_CUDA(ctx, ctx->s_wckpt.ensure(2 * lanes * BB_WIN_MAX_TILES * BB_WIN_CKPT_WORDS(BB_WIN_LW) * sizeof(uint32_t)));
+static int w_prepare(Worker &w) {
+    const bb_ctx &c = *w.ctx;
+    BB_CUDA(&w, cudaSetDevice(c.device));
+    Worker::Layout &L = w.L;
+    const int n = w.n_reads;
+    const int64_t off = w.frag_total;
+    w.seq_cap = (int64_t)((double)off * w.slack) + 16ll * n + 65536;
+    w.out_cap = w.seq_cap;
+    w.speq_cap = w.seq_cap / 32 + (2ll * BB_PEQ_PAD + 2) * n + 64;
+    L.fb_len = w.wres_total + 8;
+    BB_CUDA(&w, w.d_frag.ensure((size_t)off + 16));
+    BB_CUDA(&w, w.d_state.ensure(((size_t)off + 16) * sizeof(uint32_t)));
+    BB_CUDA(&w, w.d_kidx.ensure(((size_t)off + 16) * sizeof(int)));
+    BB_CUDA(&w, w.d_counter.ensure(BB_N_COUNTERS * sizeof(int)));
+    BB_CUDA(&w, w.d_scan.ensure(sizeof(BBScanOut)));
+    BB_CUDA(&w, w.d_levels.ensure(sizeof(Worker::RunInfo::levels)));
+    BB_CUDA(&w, w.d_fpeq.ensure(((size_t)w.fpeq_total + 4) * sizeof(uint4)));
+    BB_CUDA(&w, w.d_ctime.ensure(((size_t)off + 16) * sizeof(unsigned int)));
+    BB_CUDA(&w, w.d_chlog.ensure(((size_t)w.log_total + 16) * sizeof(uint2)));
+    BB_CUDA(&w, w.d_wres.ensure(((size_t)w.wres_total + 16) * sizeof(int2)));
+    BB_CUDA(&w, w.d_wtasks.ensure(((size_t)w.wres_total + 16) * sizeof(BBWinTask)));
+    BB_CUDA(&w, w.d_wfallback.ensure(2 * (size_t)L.fb_len * sizeof(BBWinTask)));
+    BB_CUDA(&w, w.d_seq.ensure((size_t)w.seq_cap + 16));
+    BB_CUDA(&w, w.d_ops.ensure((size_t)w.seq_cap + 16));
+    BB_CUDA(&w, w.d_dcnt.ensure(((size_t)w.seq_cap + 16) * sizeof(unsigned int)));
+    BB_CUDA(&w, w.d_qual.ensure((size_t)w.seq_cap + 16));
+    BB_CUDA(&w, w.d_speq.ensure(((size_t)w.speq_cap + 4) * sizeof(uint4)));
+    BB_CUDA(&w, w.d_out_seq.ensure((size_t)w.out_cap + 16));
+    BB_CUDA(&w, w.d_out_qual.ensure((size_t)w.out_cap + 16));
+    // Lane pools of the window aligners and the leaf aligner.  Each alignment pipeline's leaf kernel owns half of the
+    // history (checkpoints with lowmem), one lane per thread of its lane_ctas CTAs.  The window kernels run before the
+    // alignment and use the whole pool: the 4-word build up to 2 * lane_ctas CTAs, the 8-word build half as many (twice
+    // the words per lane), with lowmem both up to 2 * lane_ctas.
+    L.lane_ctas = c.sm_count * 4;
+    const size_t lanes = (size_t)L.lane_ctas * 64;
+    if (c.knobs.lowmem) {
+        L.hist_per_pipe = lanes * BB_LEAF_MAX_TILES * BB_LEAF_CKPT_WORDS;
+        BB_CUDA(&w, w.s_leafhist.ensure(2 * L.hist_per_pipe * sizeof(uint32_t)));
+    } else {
+        L.hist_per_pipe = lanes * BB_LEAF_LANE_COLS * BB_LEAF_LW;  // per-column history
+        BB_CUDA(&w, w.s_lanehist.ensure(2 * L.hist_per_pipe * sizeof(uint2)));
     }
+    BB_CUDA(&w, w.s_ltbuf.ensure(2 * lanes * BB_WIN_MAX_COLS));
+    // window aligners: a checkpoint (2 LW + 2 words) per 16 columns per lane instead of a per-column history
+    if (c.knobs.lowmem) BB_CUDA(&w, w.s_wckpt.ensure(2 * lanes * BB_WIN_MAX_TILES * BB_WIN_CKPT_WORDS(BB_WIN_LW) * sizeof(uint32_t)));
     // per-warp scratch: strip carries / bitmaps for the longest joined read; split-score arrays for the widest band
     // (expected: a few times the injected edits; worst case: the whole read; BADREAD_B200_LR_CAP replaces the expected
     // size and its floor)
-    const int len_b = (int)std::min<double>((double)ctx->max_len * ctx->slack + 64.0, (double)(1 << 24));
-    const int lr_floor = ctx->lr_cap > 0 ? ctx->lr_cap : 4096;
+    const int len_b = (int)std::min<double>((double)w.max_len * w.slack + 64.0, (double)(1 << 24));
+    const int lr_floor = c.knobs.lr_cap > 0 ? c.knobs.lr_cap : 4096;
     int lr_need = lr_floor;
     for (int r = 0; r < n; r++) {
-        const double len = (double)ctx->h_reads[(size_t)r].frag_len;
-        const double worst = len * ctx->slack + 64.0;
-        const double expect = ctx->lr_cap > 0 ? 0.0 : 3.0 * (1.0 - ctx->h_target[(size_t)r]) * len + 0.02 * len + 512.0;
-        lr_need = std::max(lr_need, (int)std::min(worst, ctx->lr_worst ? worst : expect));
+        const double len = (double)w.h_reads[(size_t)r].frag_len;
+        const double worst = len * w.slack + 64.0;
+        const double expect = c.knobs.lr_cap > 0 ? 0.0 : 3.0 * (1.0 - w.h_target[(size_t)r]) * len + 0.02 * len + 512.0;
+        lr_need = std::max(lr_need, (int)std::min(worst, w.lr_worst ? worst : expect));
     }
-    int rc = ensure_scratch(ctx, len_b, lr_need, len_b, lr_floor);
+    int rc = ensure_scratch(w, len_b, lr_need, len_b, lr_floor);
     if (rc) return rc;
-    const int cap_node = (int)std::min<int64_t>(ctx->seq_cap / 256 + 4ll * n + 1024, 0x7ffffff0);
+    int slot = 0;
+    for (int s = 0; s < 2; s++)
+        for (int k = 0; k < 3; k++) {
+            L.lean_base[s][k] = slot;
+            slot += c.sm_count * kLeanCtasPerSm[k] * BB_WARPS_PER_CTA;
+        }
+    L.cap_node = (int)std::min<int64_t>(w.seq_cap / 256 + 4ll * n + 1024, 0x7ffffff0);
     for (int s = 0; s < 2; s++) {
-        auto &qb = ctx->qbuf[s];
-        for (int c = 0; c < BBQ_NODE_CLASSES; c++)
-            for (int p = 0; p < 2; p++) BB_CUDA(ctx, qb.node[c][p].ensure((size_t)cap_node * sizeof(BBNode)));
-        for (int w = 0; w < 2; w++) BB_CUDA(ctx, qb.leaf[w].ensure((size_t)cap_node * sizeof(BBNode)));
-        BB_CUDA(ctx, qb.count.ensure(512 * sizeof(int)));
+        auto &qb = w.qbuf[s];
+        for (int k = 0; k < BBQ_NODE_CLASSES; k++)
+            for (int p = 0; p < 2; p++) BB_CUDA(&w, qb.node[k][p].ensure((size_t)L.cap_node * sizeof(BBNode)));
+        for (int x = 0; x < 2; x++) BB_CUDA(&w, qb.leaf[x].ensure((size_t)L.cap_node * sizeof(BBNode)));
+        BB_CUDA(&w, qb.count.ensure(kQueueCounts * sizeof(int)));
     }
-    ctx->n_levels = std::max(1, std::min(BB_MAX_LEVELS, level_bound(ctx->max_len, ctx->slack) + ctx->extra_levels));
+    w.n_levels = std::max(1, std::min(BB_MAX_LEVELS, level_bound(w.max_len, w.slack) + w.extra_levels));
     return BB_OK;
 }
 
-static int w_batch_upload(bb_ctx *ctx, int32_t n_reads, const uint64_t *read_index, const int32_t *seg_off,
-                          const bb_segment *segs, const uint8_t *literal_pool, int64_t literal_len,
-                          const double *target_identity) {
-    if (!ctx) return BB_ERR_ARG;
-    if (n_reads <= 0 || !read_index || !seg_off || !segs || !target_identity || literal_len < 0)
-        return set_err(ctx, BB_ERR_ARG, "bb_batch_upload: bad arguments");
-    if (!ctx->have_em || !ctx->have_qm) return set_err(ctx, BB_ERR_STATE, "upload the error and qscore models first");
-    BB_CUDA(ctx, cudaSetDevice(ctx->device));
+// Checks the descriptors of a whole batch and sums each read's segment lengths into len.
+static int check_batch(bb_ctx *ctx, int32_t n_reads, const int32_t *seg_off, const bb_segment *segs, int64_t literal_len,
+                       std::vector<int64_t> &len) {
     const int k = ctx->em.k;
-    ctx->h_reads.assign((size_t)n_reads, BBReadDev{});
-    ctx->h_inlen.assign((size_t)n_reads, 0);
-    ctx->h_target.assign(target_identity, target_identity + n_reads);
-    int64_t off = 0, peq_off = 0, log_off = 0, wres_off = 0;
-    int max_len = 0;
+    len.assign((size_t)n_reads, 0);
     for (int32_t r = 0; r < n_reads; r++) {
-        int64_t len = 0;
         if (seg_off[r + 1] < seg_off[r]) return set_err(ctx, BB_ERR_ARG, "seg_off must be non-decreasing");
         for (int32_t s = seg_off[r]; s < seg_off[r + 1]; s++) {
             const bb_segment &sg = segs[s];
@@ -648,11 +668,29 @@ static int w_batch_upload(bb_ctx *ctx, int32_t n_reads, const uint64_t *read_ind
             if (sg.kind == BB_SEG_LITERAL) { if (sg.src + sg.len > literal_len) return set_err(ctx, BB_ERR_ARG, "literal segment out of range"); }
             else if (sg.kind == BB_SEG_REF_FWD || sg.kind == BB_SEG_REF_REV) { if (sg.src + sg.len > ctx->ref_len) return set_err(ctx, BB_ERR_ARG, "reference segment out of range"); }
             else return set_err(ctx, BB_ERR_ARG, "unknown segment kind");
-            len += sg.len;
+            len[(size_t)r] += sg.len;
         }
-        if (len + 2 * k >= (1 << 24)) return set_err(ctx, BB_ERR_ARG, "fragment too long (16 Mb limit)");
-        ctx->h_inlen[(size_t)r] = (int32_t)len;
-        BBReadDev &rd = ctx->h_reads[(size_t)r];
+        if (len[(size_t)r] + 2 * k >= (1 << 24)) return set_err(ctx, BB_ERR_ARG, "fragment too long (16 Mb limit)");
+    }
+    return BB_OK;
+}
+
+// Uploads a worker's reads, whose descriptors check_batch has accepted.
+static int w_batch_upload(Worker &w, int32_t n_reads, const uint64_t *read_index, const int32_t *seg_off,
+                          const bb_segment *segs, const uint8_t *literal_pool, int64_t literal_len,
+                          const double *target_identity) {
+    BB_CUDA(&w, cudaSetDevice(w.ctx->device));
+    const int k = w.ctx->em.k;
+    w.h_reads.assign((size_t)n_reads, BBReadDev{});
+    w.h_inlen.assign((size_t)n_reads, 0);
+    w.h_target.assign(target_identity, target_identity + n_reads);
+    int64_t off = 0, peq_off = 0, log_off = 0, wres_off = 0;
+    int max_len = 0;
+    for (int32_t r = 0; r < n_reads; r++) {
+        int64_t len = 0;
+        for (int32_t s = seg_off[r]; s < seg_off[r + 1]; s++) len += segs[s].len;
+        w.h_inlen[(size_t)r] = (int32_t)len;
+        BBReadDev &rd = w.h_reads[(size_t)r];
         rd.frag_off = off;
         rd.frag_len = (int)(len + 2 * k);
         rd.fpeq_off = peq_off;
@@ -668,81 +706,82 @@ static int w_batch_upload(bb_ctx *ctx, int32_t n_reads, const uint64_t *read_ind
         off += (rd.frag_len + 15) & ~15;
         max_len = std::max(max_len, rd.frag_len);
     }
-    ctx->frag_total = off; ctx->fpeq_total = peq_off; ctx->log_total = log_off; ctx->wres_total = wres_off;
-    ctx->max_len = max_len;
+    w.frag_total = off; w.fpeq_total = peq_off; w.log_total = log_off; w.wres_total = wres_off;
+    w.max_len = max_len;
     std::vector<int> order((size_t)n_reads);
     std::iota(order.begin(), order.end(), 0);
     std::stable_sort(order.begin(), order.end(),
-                     [&](int x, int y) { return ctx->h_reads[(size_t)x].frag_len > ctx->h_reads[(size_t)y].frag_len; });
-    ctx->n_reads = n_reads;
-    ctx->h_order = order;
+                     [&](int x, int y) { return w.h_reads[(size_t)x].frag_len > w.h_reads[(size_t)y].frag_len; });
+    w.n_reads = n_reads;
+    const cudaStream_t st = w.stream;
     int rc;
-    if ((rc = upload(ctx, ctx->d_read_index, read_index, (size_t)n_reads))) return rc;
-    if ((rc = upload(ctx, ctx->d_seg_off, seg_off, (size_t)n_reads + 1))) return rc;
-    if ((rc = upload(ctx, ctx->d_segs, segs, (size_t)seg_off[n_reads]))) return rc;
-    if ((rc = upload(ctx, ctx->d_lit, literal_pool, (size_t)literal_len))) return rc;
-    if ((rc = upload(ctx, ctx->d_target, target_identity, (size_t)n_reads))) return rc;
-    if ((rc = upload(ctx, ctx->d_order, order.data(), (size_t)n_reads))) return rc;
-    if ((rc = upload(ctx, ctx->d_reads, ctx->h_reads.data(), (size_t)n_reads))) return rc;
-    if ((rc = w_prepare(ctx))) return rc;
-    BB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    ctx->uploaded = true;
-    ctx->ran = false;
-    ctx->finished = false;
+    if ((rc = upload(&w, st, w.d_read_index, read_index, (size_t)n_reads))) return rc;
+    if ((rc = upload(&w, st, w.d_seg_off, seg_off, (size_t)n_reads + 1))) return rc;
+    if ((rc = upload(&w, st, w.d_segs, segs, (size_t)seg_off[n_reads]))) return rc;
+    if ((rc = upload(&w, st, w.d_lit, literal_pool, (size_t)literal_len))) return rc;
+    if ((rc = upload(&w, st, w.d_target, target_identity, (size_t)n_reads))) return rc;
+    if ((rc = upload(&w, st, w.d_order, order.data(), (size_t)n_reads))) return rc;
+    if ((rc = upload(&w, st, w.d_reads, w.h_reads.data(), (size_t)n_reads))) return rc;
+    if ((rc = w_prepare(w))) return rc;
+    BB_CUDA(&w, cudaStreamSynchronize(st));
+    w.uploaded = true;
+    w.ran = false;
+    w.finished = false;
     return BB_OK;
 }
 
-// Persistent grids (CTAs that pull work from a queue until it is empty) of `per_sm` CTAs per SM at full size.  The
-// workers of a split batch run side by side: each launches its share, so that their kernels are resident together
-// instead of queueing behind each other's long-running CTAs.
-static int pgrid(const bb_ctx *ctx, int per_sm, const char *knob = nullptr) {
-    if (knob) {  // tuning: BADREAD_B200_GRID_<KNOB> = CTAs per SM of that kernel
-        static thread_local char name[64];
-        std::snprintf(name, sizeof(name), "BADREAD_B200_GRID_%s", knob);
-        if (const char *e = std::getenv(name)) { const int v = std::atoi(e); if (v > 0) per_sm = v; }
-    }
-    return std::max(ctx->sm_count / 2, (ctx->sm_count * per_sm + ctx->grid_div - 1) / ctx->grid_div);
+// Persistent grids (CTAs that pull work from a queue until it is empty) of `per_sm` CTAs per SM at full size, or of
+// the GRID_<knob> setting.  The workers of a split batch run side by side: each launches its share (GRID_DIV; all of
+// the SMs by default), so that their kernels are resident together instead of queueing behind each other's CTAs.
+static int pgrid(const Worker &w, int per_sm, int knob = kGridKnobs) {
+    const bb_ctx &c = *w.ctx;
+    if (knob < kGridKnobs && c.knobs.grid[knob] > 0) per_sm = c.knobs.grid[knob];
+    const int div = c.n_split > 1 && c.knobs.grid_div > 0 ? c.knobs.grid_div : 1;
+    return std::max(c.sm_count / 2, (c.sm_count * per_sm + div - 1) / div);
 }
 
 // The error loop decoupled from its identity re-measurements (bb_loop.cuh): mutate ahead -> task list -> all window
 // alignments as independent lane tasks -> scalar replay, n_rounds times back to back.  A round after the last read
 // has finished costs six launches that find nothing to do; a read that is still pending after the last round is
 // reported by the replay kernel's counter and w_finish runs the batch again with more rounds.
-static int enqueue_error_loop(bb_ctx *ctx, const BBBatchDev &B) {
-    cudaStream_t st = ctx->stream;
-    const int n = ctx->n_reads;
-    int *cnt = ctx->d_counter.as<int>();
-    const int lane_ctas = ctx->sm_count * 4;
-    const int *order = ctx->d_order.as<int>();
-    BBWinTask *tasks = ctx->d_wtasks.as<BBWinTask>();
-    BBWinTask *fb1 = ctx->d_wfallback.as<BBWinTask>(), *fb2 = fb1 + ctx->wres_total + 8;
-    for (int round = 0; round < ctx->n_rounds; round++) {
-        int *c = cnt + BB_ROUND_BASE(round);
-        bbl_mutate(std::min(pgrid(ctx, 8, "MUTATE"), n), st, B, ctx->em, ctx->seed, c + BBC_MUTATE, order, n, ctx->is_head);
-        mark(ctx, st, "mutate");
-        bb_k_window_tasks<<<(n + 255) / 256, 256, 0, st>>>(B, order, n, tasks, c + BBC_NTASKS);
-        mark(ctx, st, "window_tasks");
+static int enqueue_error_loop(Worker &w, const BBBatchDev &B) {
+    const bb_ctx &c = *w.ctx;
+    const Worker::Layout &L = w.L;
+    const BBErrorModelDev &em = c.em;
+    cudaStream_t st = w.stream;
+    const int n = w.n_reads;
+    const int win_grid = 2 * L.lane_ctas;  // what the lane pools hold (see w_prepare)
+    int *cnt = w.d_counter.as<int>();
+    const int *order = w.d_order.as<int>();
+    BBWinTask *tasks = w.d_wtasks.as<BBWinTask>();
+    BBWinTask *fb1 = w.d_wfallback.as<BBWinTask>(), *fb2 = fb1 + L.fb_len;
+    for (int round = 0; round < w.n_rounds; round++) {
+        int *cr = cnt + BB_ROUND_BASE(round);
+        bbl_mutate(std::min(pgrid(w, 8, G_MUTATE), n), st, B, em, c.seed, cr + BBC_MUTATE, order, n, w.is_head);
+        mark(w, st, "mutate");
+        bb_k_window_tasks<<<(n + 255) / 256, 256, 0, st>>>(B, order, n, tasks, cr + BBC_NTASKS);
+        mark(w, st, "window_tasks");
         // 4-word windows first (bands up to 64 rows: almost every window); what does not fit falls through to the
         // 8-word build and from there to the warp kernel
-        if (ctx->lowmem)
-            bbl_window_lane4(std::min(pgrid(ctx, 6, "WIN4"), ctx->sm_count * 8), st, B, ctx->em, tasks, c + BBC_NTASKS, ctx->seed,
-                             ctx->s_wckpt.as<uint32_t>(), ctx->s_ltbuf.as<uint8_t>(), c + BBC_LANE4, fb1, c + BBC_FB1);
+        if (c.knobs.lowmem)
+            bbl_window_lane4(std::min(pgrid(w, 6, G_WIN4), win_grid), st, B, em, tasks, cr + BBC_NTASKS, c.seed,
+                             w.s_wckpt.as<uint32_t>(), w.s_ltbuf.as<uint8_t>(), cr + BBC_LANE4, fb1, cr + BBC_FB1);
         else
-            bbl_window_lane_hist(4, ctx->ring_t, std::min(pgrid(ctx, 8, "WIN4"), ctx->sm_count * 8), st, B, ctx->em, tasks, c + BBC_NTASKS,
-                                 ctx->seed, ctx->s_lanehist.as<uint2>(), ctx->s_ltbuf.as<uint8_t>(), c + BBC_LANE4, fb1, c + BBC_FB1);
-        mark(ctx, st, "window_lane4");
-        if (ctx->lowmem)
-            bbl_window_lane8(std::min(pgrid(ctx, 3, "WIN8"), ctx->sm_count * 8), st, B, ctx->em, fb1, c + BBC_FB1, ctx->seed,
-                             ctx->s_wckpt.as<uint32_t>(), ctx->s_ltbuf.as<uint8_t>(), c + BBC_LANE8, fb2, c + BBC_FB2);
+            bbl_window_lane_hist(4, c.knobs.ring_t, std::min(pgrid(w, 8, G_WIN4), win_grid), st, B, em, tasks, cr + BBC_NTASKS,
+                                 c.seed, w.s_lanehist.as<uint2>(), w.s_ltbuf.as<uint8_t>(), cr + BBC_LANE4, fb1, cr + BBC_FB1);
+        mark(w, st, "window_lane4");
+        if (c.knobs.lowmem)
+            bbl_window_lane8(std::min(pgrid(w, 3, G_WIN8), win_grid), st, B, em, fb1, cr + BBC_FB1, c.seed,
+                             w.s_wckpt.as<uint32_t>(), w.s_ltbuf.as<uint8_t>(), cr + BBC_LANE8, fb2, cr + BBC_FB2);
         else
-            bbl_window_lane_hist(8, 4, std::min(pgrid(ctx, 4, "WIN8"), ctx->sm_count * 4), st, B, ctx->em, fb1, c + BBC_FB1, ctx->seed,
-                                 ctx->s_lanehist.as<uint2>(), ctx->s_ltbuf.as<uint8_t>(), c + BBC_LANE8, fb2, c + BBC_FB2);
-        mark(ctx, st, "window_lane8");
-        bbl_window_warp(pgrid(ctx, 2), st, B, ctx->em, ctx->pool, fb2, c + BBC_FB2, ctx->seed, c + BBC_WARP);
-        mark(ctx, st, "window_warp");
-        bb_k_replay<<<(n + 3) / 4, 128, 0, st>>>(B, order, n, ctx->em.k, c + BBC_PENDING);
-        mark(ctx, st, "replay");
-        ctx->launches += 6;
+            bbl_window_lane_hist(8, 4, std::min(pgrid(w, 4, G_WIN8), win_grid / 2), st, B, em, fb1, cr + BBC_FB1, c.seed,
+                                 w.s_lanehist.as<uint2>(), w.s_ltbuf.as<uint8_t>(), cr + BBC_LANE8, fb2, cr + BBC_FB2);
+        mark(w, st, "window_lane8");
+        bbl_window_warp(pgrid(w, 2), st, B, em, w.pool, fb2, cr + BBC_FB2, c.seed, cr + BBC_WARP);
+        mark(w, st, "window_warp");
+        bb_k_replay<<<(n + 3) / 4, 128, 0, st>>>(B, order, n, em.k, cr + BBC_PENDING);
+        mark(w, st, "replay");
+        w.launches += 6;
     }
     return BB_OK;
 }
@@ -750,206 +789,204 @@ static int enqueue_error_loop(bb_ctx *ctx, const BBBatchDev &B) {
 // Final alignment as level-synchronous tasks (bb_tasks.cuh): every level of all reads' Hirschberg trees is a few
 // launches (warp-pair, lean-warp and lane nodes), leaves run at the end.  The number of levels comes from the longest
 // fragment; nodes left over after the last level are reported by the queue counters (w_finish adds levels).
-static int enqueue_align_tasks(bb_ctx *ctx, const BBBatchDev &B) {
-    cudaStream_t stream[2] = {ctx->stream, ctx->stream2};
-    const int n = ctx->n_reads;
-    const int cap_node = (int)std::min<int64_t>(ctx->seq_cap / 256 + 4ll * n + 1024, 0x7ffffff0);
-    const int lane_ctas = ctx->sm_count * 4;
-    const size_t hist_per_pipe = (size_t)lane_ctas * 64 * BB_LEAF_MAX_TILES * BB_LEAF_CKPT_WORDS;  // checkpoint words
+static int enqueue_align_tasks(Worker &w, const BBBatchDev &B) {
+    const bb_ctx &c = *w.ctx;
+    const Knobs &kn = c.knobs;
+    const Worker::Layout &L = w.L;
+    cudaStream_t stream[2] = {w.stream, w.stream2};
+    const int n = w.n_reads;
     BBQueues Q[2];
     int *cnt[2];
     for (int s = 0; s < 2; s++) {
-        auto &qb = ctx->qbuf[s];
-        for (int c = 0; c < BBQ_NODE_CLASSES; c++)
-            for (int p = 0; p < 2; p++) Q[s].node[c][p] = qb.node[c][p].as<BBNode>();
-        for (int w = 0; w < 2; w++) Q[s].leaf[w] = qb.leaf[w].as<BBNode>();
+        auto &qb = w.qbuf[s];
+        for (int k = 0; k < BBQ_NODE_CLASSES; k++)
+            for (int p = 0; p < 2; p++) Q[s].node[k][p] = qb.node[k][p].as<BBNode>();
+        for (int x = 0; x < 2; x++) Q[s].leaf[x] = qb.leaf[x].as<BBNode>();
         cnt[s] = qb.count.as<int>();
-        Q[s].count = cnt[s]; Q[s].overflow = cnt[s] + BBQ_OVERFLOW; Q[s].cap_node = cap_node; Q[s].cap_leaf = cap_node;
-        Q[s].lane8_cols = ctx->lane8_cols;
-        BB_CUDA(ctx, cudaMemsetAsync(cnt[s], 0, 512 * sizeof(int), stream[0]));
+        Q[s].count = cnt[s]; Q[s].overflow = cnt[s] + BBQ_OVERFLOW; Q[s].cap_node = L.cap_node; Q[s].cap_leaf = L.cap_node;
+        Q[s].lane8_cols = kn.lane8_cols;
+        BB_CUDA(&w, cudaMemsetAsync(cnt[s], 0, kQueueCounts * sizeof(int), stream[0]));
     }
-    int *snap = ctx->d_levels.as<int>();
-    BB_CUDA(ctx, cudaMemsetAsync(snap, 0, sizeof(bb_ctx::RunInfo::levels), stream[0]));
-    bb_k_push_roots<<<(n + 255) / 256, 256, 0, stream[0]>>>(B, Q[0], Q[1], ctx->d_order.as<int>());
-    ctx->launches++;
+    int *snap = w.d_levels.as<int>();
+    BB_CUDA(&w, cudaMemsetAsync(snap, 0, sizeof(Worker::RunInfo::levels), stream[0]));
+    bb_k_push_roots<<<(n + 255) / 256, 256, 0, stream[0]>>>(B, Q[0], Q[1], w.d_order.as<int>());
+    w.launches++;
     // pipeline 0 (stream 0): every read whose root band fits the lean / lane kernels; pipeline 1 (stream 1): reads
     // with a wide root (long or noisy reads).  The two never wait for each other's levels.
-    BB_CUDA(ctx, cudaEventRecord(ctx->ev_fork, stream[0]));
-    BB_CUDA(ctx, cudaStreamWaitEvent(stream[1], ctx->ev_fork, 0));
-    int *cursor[2] = {cnt[0] + 16, cnt[1] + 16};
-    const int warp_base[2] = {0, ctx->n_warps / 2};
-    const int w4 = ctx->sm_count * 4 * BB_WARPS_PER_CTA, w2 = ctx->sm_count * 6 * BB_WARPS_PER_CTA;  // scratch slots of the lean kernels (maxima)
-    const int lean_base[2] = {0, w4 + 2 * w2};
+    BB_CUDA(&w, cudaEventRecord(w.ev_fork, stream[0]));
+    BB_CUDA(&w, cudaStreamWaitEvent(stream[1], w.ev_fork, 0));
+    int *cursor[2] = {cnt[0] + kCursorBase, cnt[1] + kCursorBase};
+    const int warp_base[2] = {0, c.n_warps / 2};
     // The node classes of a level read the same queues and push into the next level's: they are independent and run
     // side by side on their own streams; the level ends when all of them have finished.
-    for (int level = 0; level < ctx->n_levels; level++) {
+    for (int level = 0; level < w.n_levels; level++) {
         // (the roots are queued longest read first; every later queue fills in the order the parents finish, longest
         // last, and is walked from its end)
-        const int p = (level & 1) | (level > 0 && ctx->lpt_order ? BBQ_BACKWARDS : 0);
+        const int p = (level & 1) | (level > 0 && kn.lpt_order ? BBQ_BACKWARDS : 0);
         for (int s = 0; s < 2; s++) {
             cudaStream_t st = stream[s];
             // this level's node counts are final here and cleared when the next level starts: keep them
             // (bb_last_run_work); the leaf counters at level 0 are the roots' leaves
             int *row = snap + (s * BB_MAX_LEVELS + level) * BB_SNAP_WORDS;
-            BB_CUDA(ctx, cudaMemcpyAsync(row, cnt[s] + BBQ_COUNT(0, p & 1), BBQ_NODE_CLASSES * sizeof(int), cudaMemcpyDeviceToDevice, st));
+            BB_CUDA(&w, cudaMemcpyAsync(row, cnt[s] + BBQ_COUNT(0, p & 1), BBQ_NODE_CLASSES * sizeof(int), cudaMemcpyDeviceToDevice, st));
             if (level == 0)
-                BB_CUDA(ctx, cudaMemcpyAsync(row + BB_SNAP_LEAF, cnt[s] + BBQ_LEAF_COUNT, 2 * sizeof(int), cudaMemcpyDeviceToDevice, st));
-            BB_CUDA(ctx, cudaMemsetAsync(cnt[s] + BBQ_COUNT(0, (p & 1) ^ 1), 0, BBQ_NODE_CLASSES * sizeof(int), st));
-            BB_CUDA(ctx, cudaEventRecord(ctx->ev_level[s], st));
+                BB_CUDA(&w, cudaMemcpyAsync(row + BB_SNAP_LEAF, cnt[s] + BBQ_LEAF_COUNT, 2 * sizeof(int), cudaMemcpyDeviceToDevice, st));
+            BB_CUDA(&w, cudaMemsetAsync(cnt[s] + BBQ_COUNT(0, (p & 1) ^ 1), 0, BBQ_NODE_CLASSES * sizeof(int), st));
+            BB_CUDA(&w, cudaEventRecord(w.ev_level[s], st));
             int n_side = 0;
             auto on_side = [&]() -> cudaStream_t {
-                cudaStream_t x = ctx->side[s][n_side++];
-                cudaStreamWaitEvent(x, ctx->ev_level[s], 0);
-                mark(ctx, x, "fork");
+                cudaStream_t x = w.side[s][n_side++];
+                cudaStreamWaitEvent(x, w.ev_level[s], 0);
+                mark(w, x, "fork");
                 return x;
             };
             if (s == 1) {
                 cudaStream_t x = on_side();
-                if (ctx->use_quad) bbl_node_quad(ctx->sm_count, x, B, Q[s], ctx->pool, p, cursor[s]++, warp_base[s]);
-                else bbl_node_pair(ctx->sm_count * ctx->pair_ctas, x, B, Q[s], ctx->pool, p, cursor[s]++, warp_base[s]);
-                ctx->launches++;
-                mark(ctx, x, ctx->use_quad ? "node_quad" : "node_pair");
+                if (kn.use_quad) bbl_node_quad(c.sm_count, x, B, Q[s], w.pool, p, cursor[s]++, warp_base[s]);
+                else bbl_node_pair(c.sm_count * kn.pair_ctas, x, B, Q[s], w.pool, p, cursor[s]++, warp_base[s]);
+                w.launches++;
+                mark(w, x, kn.use_quad ? "node_quad" : "node_pair");
             }
             {
                 cudaStream_t x = on_side();   // the two narrow single-warp classes share a stream
-                bbl_node_warp(2, std::min(pgrid(ctx, 3, "WARP2"), ctx->sm_count * 6), x, B, Q[s], ctx->pool_lean, p, cursor[s]++, lean_base[s] + w4);
-                mark(ctx, x, "node_warp2");
-                bbl_node_warp(1, std::min(pgrid(ctx, 3, "WARP1"), ctx->sm_count * 6), x, B, Q[s], ctx->pool_lean, p, cursor[s]++, lean_base[s] + w4 + w2);
-                mark(ctx, x, "node_warp1");
+                bbl_node_warp(2, std::min(pgrid(w, 3, G_WARP2), c.sm_count * kLeanCtasPerSm[LEAN2]), x, B, Q[s], w.pool_lean, p, cursor[s]++,
+                              L.lean_base[s][LEAN2]);
+                mark(w, x, "node_warp2");
+                bbl_node_warp(1, std::min(pgrid(w, 3, G_WARP1), c.sm_count * kLeanCtasPerSm[LEAN1]), x, B, Q[s], w.pool_lean, p, cursor[s]++,
+                              L.lean_base[s][LEAN1]);
+                mark(w, x, "node_warp1");
                 x = on_side();
-                bbl_node_lane8(pgrid(ctx, 6, "LANE8"), x, B, Q[s], p, cursor[s]++);
-                mark(ctx, x, "node_lane8");
+                bbl_node_lane8(pgrid(w, 6, G_LANE8), x, B, Q[s], p, cursor[s]++);
+                mark(w, x, "node_lane8");
             }
-            bbl_node_warp(4, std::min(pgrid(ctx, 2, "WARP4"), ctx->sm_count * 4), st, B, Q[s], ctx->pool_lean, p, cursor[s]++, lean_base[s]);
-            mark(ctx, st, "node_warp4");
-            ctx->launches += 4;
+            bbl_node_warp(4, std::min(pgrid(w, 2, G_WARP4), c.sm_count * kLeanCtasPerSm[LEAN4]), st, B, Q[s], w.pool_lean, p, cursor[s]++,
+                          L.lean_base[s][LEAN4]);
+            mark(w, st, "node_warp4");
+            w.launches += 4;
             for (int x = 0; x < n_side; x++) {
-                BB_CUDA(ctx, cudaEventRecord(ctx->ev_side[s][x], ctx->side[s][x]));
-                BB_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev_side[s][x], 0));
+                BB_CUDA(&w, cudaEventRecord(w.ev_side[s][x], w.side[s][x]));
+                BB_CUDA(&w, cudaStreamWaitEvent(st, w.ev_side[s][x], 0));
             }
         }
     }
     for (int s = 0; s < 2; s++) {
         cudaStream_t st = stream[s];
-        bbl_leaf_warp(ctx->sm_count, st, B, Q[s], ctx->pool, cursor[s]++, warp_base[s]);
-        mark(ctx, st, "leaf_warp");
-        if (ctx->lowmem)
-            bbl_leaf_lane(std::min(pgrid(ctx, 3, "LEAF"), ctx->sm_count * 4), st, B, Q[s], ctx->s_leafhist.as<uint32_t>() + s * hist_per_pipe, cursor[s]++);
+        bbl_leaf_warp(c.sm_count, st, B, Q[s], w.pool, cursor[s]++, warp_base[s]);
+        mark(w, st, "leaf_warp");
+        if (kn.lowmem)
+            bbl_leaf_lane(std::min(pgrid(w, 3, G_LEAF), L.lane_ctas), st, B, Q[s], w.s_leafhist.as<uint32_t>() + s * L.hist_per_pipe, cursor[s]++);
         else
-            bbl_leaf_lane_hist(std::min(pgrid(ctx, 4, "LEAF"), ctx->sm_count * 4), st, B, Q[s],
-                               ctx->s_lanehist.as<uint2>() + s * ((size_t)lane_ctas * 64 * BB_LEAF_LANE_COLS * BB_LEAF_LW), cursor[s]++);
-        mark(ctx, st, "leaf_lane");
-        ctx->launches += 2;
+            bbl_leaf_lane_hist(std::min(pgrid(w, 4, G_LEAF), L.lane_ctas), st, B, Q[s], w.s_lanehist.as<uint2>() + s * L.hist_per_pipe, cursor[s]++);
+        mark(w, st, "leaf_lane");
+        w.launches += 2;
     }
-    BB_CUDA(ctx, cudaEventRecord(ctx->ev_join, stream[1]));
-    BB_CUDA(ctx, cudaStreamWaitEvent(stream[0], ctx->ev_join, 0));
+    BB_CUDA(&w, cudaEventRecord(w.ev_join, stream[1]));
+    BB_CUDA(&w, cudaStreamWaitEvent(stream[0], w.ev_join, 0));
     for (int s = 0; s < 2; s++)
-        BB_CUDA(ctx, cudaMemcpyAsync(ctx->h_info->qcount[s], cnt[s], 32 * sizeof(int), cudaMemcpyDeviceToHost, stream[0]));
-    BB_CUDA(ctx, cudaMemcpyAsync(ctx->h_info->levels, snap, sizeof(bb_ctx::RunInfo::levels), cudaMemcpyDeviceToHost, stream[0]));
+        BB_CUDA(&w, cudaMemcpyAsync(w.h_info->qcount[s], cnt[s], 32 * sizeof(int), cudaMemcpyDeviceToHost, stream[0]));
+    BB_CUDA(&w, cudaMemcpyAsync(w.h_info->levels, snap, sizeof(Worker::RunInfo::levels), cudaMemcpyDeviceToHost, stream[0]));
     return BB_OK;
 }
 
 // Enqueues the whole hot path of the uploaded batch on the worker's streams and returns: no host round trip inside.
-static int w_enqueue(bb_ctx *ctx) {
-    if (!ctx) return BB_ERR_ARG;
-    if (!ctx->uploaded) return set_err(ctx, BB_ERR_STATE, "bb_batch_run: no batch uploaded");
-    BB_CUDA(ctx, cudaSetDevice(ctx->device));
-    cudaStream_t st = ctx->stream;
-    const int n = ctx->n_reads;
-    BBBatchDev B = batch_dev(ctx);
-    ctx->finished = false;
+static int w_enqueue(Worker &w) {
+    if (!w.uploaded) return set_err(&w, BB_ERR_STATE, "bb_batch_run: no batch uploaded");
+    const bb_ctx &c = *w.ctx;
+    BB_CUDA(&w, cudaSetDevice(c.device));
+    cudaStream_t st = w.stream;
+    const int n = w.n_reads;
+    BBBatchDev B = batch_dev(w);
+    w.finished = false;
     // the per-read records start from the uploaded state on every run (bb_batch_run may be repeated)
-    BB_CUDA(ctx, cudaMemcpyAsync(ctx->d_reads.p, ctx->h_reads.data(), (size_t)n * sizeof(BBReadDev), cudaMemcpyHostToDevice, st));
-    BB_CUDA(ctx, cudaMemsetAsync(ctx->d_counter.p, 0, BB_N_COUNTERS * sizeof(int), st));
-    ctx->marks.clear(); ctx->mark_used = 0;
-    mark(ctx, st, "begin");
-    BB_CUDA(ctx, cudaEventRecord(ctx->ev[0], st));
-    if (ctx->em.type == 1 && ctx->em_hash.entries)
-        bb_k_build_fragments<0, true><<<n, 256, 0, st>>>(B, ctx->ref.as<uint8_t>(), ctx->em.k, ctx->seed, nullptr, ctx->em_hash);
+    BB_CUDA(&w, cudaMemcpyAsync(w.d_reads.p, w.h_reads.data(), (size_t)n * sizeof(BBReadDev), cudaMemcpyHostToDevice, st));
+    BB_CUDA(&w, cudaMemsetAsync(w.d_counter.p, 0, BB_N_COUNTERS * sizeof(int), st));
+    w.marks.clear(); w.mark_used = 0;
+    mark(w, st, "begin");
+    BB_CUDA(&w, cudaEventRecord(w.ev[0], st));
+    if (c.em.type == 1 && c.em_hash.entries)
+        bb_k_build_fragments<0, true><<<n, 256, 0, st>>>(B, c.ref.as<uint8_t>(), c.em.k, c.seed, nullptr, c.em_hash);
     else
-        bb_k_build_fragments<<<n, 256, 0, st>>>(B, ctx->ref.as<uint8_t>(), ctx->em.k, ctx->seed,
-                                                 ctx->em.type == 1 ? ctx->em.kmer_to_row : nullptr);
-    ctx->launches++;
-    mark(ctx, st, "build_fragments");
-    BB_CUDA(ctx, cudaEventRecord(ctx->ev[1], st));
-    int rc = enqueue_error_loop(ctx, B);
+        bb_k_build_fragments<<<n, 256, 0, st>>>(B, c.ref.as<uint8_t>(), c.em.k, c.seed,
+                                                 c.em.type == 1 ? c.em.kmer_to_row : nullptr);
+    w.launches++;
+    mark(w, st, "build_fragments");
+    BB_CUDA(&w, cudaEventRecord(w.ev[1], st));
+    int rc = enqueue_error_loop(w, B);
     if (rc) return rc;
-    BB_CUDA(ctx, cudaEventRecord(ctx->ev[2], st));
+    BB_CUDA(&w, cudaEventRecord(w.ev[2], st));
     // offsets of the per-read regions of the joined reads, on the device
-    bb_k_scan<<<1, 1024, 0, st>>>(B, n, ctx->seq_cap, ctx->out_cap, ctx->speq_cap, ctx->d_scan.as<BBScanOut>());
-    ctx->launches++;
-    BB_CUDA(ctx, cudaMemcpyAsync(&ctx->h_info->scan, ctx->d_scan.p, sizeof(BBScanOut), cudaMemcpyDeviceToHost, st));
-    BB_CUDA(ctx, cudaEventRecord(ctx->ev_scan, st));  // from here on the host can learn the size of this worker's output
-    BB_CUDA(ctx, cudaMemsetAsync(ctx->d_dcnt.p, 0, ((size_t)ctx->seq_cap + 16) * sizeof(unsigned int), st));
-    mark(ctx, st, "scan");
-    BB_CUDA(ctx, cudaEventRecord(ctx->ev[3], st));
-    bb_k_join<<<n, 256, 0, st>>>(B, ctx->em);
-    ctx->launches++;
-    mark(ctx, st, "join");
-    BB_CUDA(ctx, cudaEventRecord(ctx->ev[4], st));
-    if ((rc = enqueue_align_tasks(ctx, B))) return rc;
-    mark(ctx, st, "align_tail");
-    BB_CUDA(ctx, cudaEventRecord(ctx->ev[5], st));
-    bb_k_qscores<<<n, 256, 0, st>>>(B, ctx->qm, ctx->seed);
-    ctx->launches++;
-    mark(ctx, st, "qscores");
-    BB_CUDA(ctx, cudaEventRecord(ctx->ev[6], st));
+    bb_k_scan<<<1, 1024, 0, st>>>(B, n, w.seq_cap, w.out_cap, w.speq_cap, w.d_scan.as<BBScanOut>());
+    w.launches++;
+    BB_CUDA(&w, cudaMemcpyAsync(&w.h_info->scan, w.d_scan.p, sizeof(BBScanOut), cudaMemcpyDeviceToHost, st));
+    BB_CUDA(&w, cudaEventRecord(w.ev_scan, st));  // from here on the host can learn the size of this worker's output
+    BB_CUDA(&w, cudaMemsetAsync(w.d_dcnt.p, 0, ((size_t)w.seq_cap + 16) * sizeof(unsigned int), st));
+    mark(w, st, "scan");
+    BB_CUDA(&w, cudaEventRecord(w.ev[3], st));
+    bb_k_join<<<n, 256, 0, st>>>(B, c.em);
+    w.launches++;
+    mark(w, st, "join");
+    BB_CUDA(&w, cudaEventRecord(w.ev[4], st));
+    if ((rc = enqueue_align_tasks(w, B))) return rc;
+    mark(w, st, "align_tail");
+    BB_CUDA(&w, cudaEventRecord(w.ev[5], st));
+    bb_k_qscores<<<n, 256, 0, st>>>(B, c.qm, c.seed);
+    w.launches++;
+    mark(w, st, "qscores");
+    BB_CUDA(&w, cudaEventRecord(w.ev[6], st));
     bb_k_compact<<<n, 256, 0, st>>>(B);
-    ctx->launches++;
-    mark(ctx, st, "compact");
-    BB_CUDA(ctx, cudaEventRecord(ctx->ev[7], st));
-    BB_CUDA(ctx, cudaMemcpyAsync(ctx->h_info->counters, ctx->d_counter.p, BB_N_COUNTERS * sizeof(int), cudaMemcpyDeviceToHost, st));
-    BB_CUDA(ctx, cudaGetLastError());
-    ctx->ran = true;
+    w.launches++;
+    mark(w, st, "compact");
+    BB_CUDA(&w, cudaEventRecord(w.ev[7], st));
+    BB_CUDA(&w, cudaMemcpyAsync(w.h_info->counters, w.d_counter.p, BB_N_COUNTERS * sizeof(int), cudaMemcpyDeviceToHost, st));
+    BB_CUDA(&w, cudaGetLastError());
+    w.ran = true;
     return BB_OK;
 }
 
 // Waits for the worker's run and checks what the device reported.  Returns BB_OK when the results are final; when
 // something did not fit (buffers sized from the fragment lengths, rounds, levels, split-score scratch) the knob is
 // raised and the batch runs again - the results do not depend on any of them.
-static int w_finish(bb_ctx *ctx) {
-    if (!ctx) return BB_ERR_ARG;
-    if (!ctx->ran) return set_err(ctx, BB_ERR_STATE, "no run to finish");
-    if (ctx->finished) return BB_OK;
-    BB_CUDA(ctx, cudaSetDevice(ctx->device));
-    const int n = ctx->n_reads;
+static int w_finish(Worker &w) {
+    if (!w.ran) return set_err(&w, BB_ERR_STATE, "no run to finish");
+    if (w.finished) return BB_OK;
+    BB_CUDA(&w, cudaSetDevice(w.ctx->device));
+    const int n = w.n_reads;
     for (int attempt = 0;; attempt++) {
-        ctx->h_res.resize((size_t)n);
-        BB_CUDA(ctx, cudaMemcpyAsync(ctx->h_res.data(), ctx->d_reads.p, (size_t)n * sizeof(BBReadDev), cudaMemcpyDeviceToHost, ctx->stream));
-        BB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        const bb_ctx::RunInfo &info = *ctx->h_info;
+        w.h_res.resize((size_t)n);
+        BB_CUDA(&w, cudaMemcpyAsync(w.h_res.data(), w.d_reads.p, (size_t)n * sizeof(BBReadDev), cudaMemcpyDeviceToHost, w.stream));
+        BB_CUDA(&w, cudaStreamSynchronize(w.stream));
+        const Worker::RunInfo &info = *w.h_info;
         uint32_t again = 0;
         std::string why;
-        if (info.counters[BB_ROUND_BASE(ctx->n_rounds - 1) + BBC_PENDING] > 0 || info.scan.n_pending > 0) {
-            ctx->n_rounds = std::min(BB_MAX_ROUNDS, ctx->n_rounds + 3); again |= BB_RERUN_ROUNDS; why += " error-loop rounds";
+        if (info.counters[BB_ROUND_BASE(w.n_rounds - 1) + BBC_PENDING] > 0 || info.scan.n_pending > 0) {
+            w.n_rounds = std::min(BB_MAX_ROUNDS, w.n_rounds + 3); again |= BB_RERUN_ROUNDS; why += " error-loop rounds";
         }
         if (info.scan.n_nospace > 0) {  // (reads still pending after the last round are counted separately)
-            const double need = (double)std::max(info.scan.seq_total, info.scan.out_total) / (double)std::max<int64_t>(1, ctx->frag_total);
-            ctx->slack = std::max(ctx->slack * 1.5, need * 1.1 + 0.05); again |= BB_RERUN_SLACK; why += " buffer slack";
+            const double need = (double)std::max(info.scan.seq_total, info.scan.out_total) / (double)std::max<int64_t>(1, w.frag_total);
+            w.slack = std::max(w.slack * 1.5, need * 1.1 + 0.05); again |= BB_RERUN_SLACK; why += " buffer slack";
         }
-        const int last_parity = ctx->n_levels & 1;  // the queues the level after the last one would read
+        const int last_parity = w.n_levels & 1;  // the queues the level after the last one would read
         int left = 0, overflow = 0;
         for (int s = 0; s < 2; s++) {
             for (int c = 0; c < BBQ_NODE_CLASSES; c++) left += info.qcount[s][BBQ_COUNT(c, last_parity)];
             overflow += info.qcount[s][BBQ_OVERFLOW];
         }
-        if (left > 0) { ctx->extra_levels += 8; again |= BB_RERUN_LEVELS; why += " levels"; }
-        if (overflow) { ctx->slack *= 1.5; again |= BB_RERUN_QUEUES; why += " task queues"; }
-        for (int r = 0; r < n && !ctx->lr_worst; r++) {
-            const int f = (ctx->h_res[(size_t)r].flags & ~BB_FLAG_NOSPACE) >> 8;
-            if (f & (16 | 4 | 2)) { ctx->lr_worst = true; ctx->slack *= 1.25; again |= BB_RERUN_SCRATCH; why += " alignment scratch"; }
+        if (left > 0) { w.extra_levels += 8; again |= BB_RERUN_LEVELS; why += " levels"; }
+        if (overflow) { w.slack *= 1.5; again |= BB_RERUN_QUEUES; why += " task queues"; }
+        for (int r = 0; r < n && !w.lr_worst; r++) {
+            const int f = (w.h_res[(size_t)r].flags & ~BB_FLAG_NOSPACE) >> 8;
+            if (f & (16 | 4 | 2)) { w.lr_worst = true; w.slack *= 1.25; again |= BB_RERUN_SCRATCH; why += " alignment scratch"; }
         }
         if (!again) break;
-        ctx->reran = true;
-        ctx->rerun_reasons |= again;
-        if (attempt >= 3) return set_err(ctx, BB_ERR_INTERNAL, "batch did not fit after growing:" + why);
-        ctx->n_reruns++;
-        int rc = w_prepare(ctx);
+        w.reran = true;
+        w.rerun_reasons |= again;
+        if (attempt >= 3) return set_err(&w, BB_ERR_INTERNAL, "batch did not fit after growing:" + why);
+        w.n_reruns++;
+        int rc = w_prepare(w);
         if (rc) return rc;
-        if ((rc = w_enqueue(ctx))) return rc;
+        if ((rc = w_enqueue(w))) return rc;
     }
-    ctx->out_total = ctx->h_info->scan.out_total;
-    ctx->finished = true;
+    w.finished = true;
     return BB_OK;
 }
 
@@ -967,45 +1004,31 @@ extern "C" int bb_host_free(void *ptr) {
 extern "C" int bb_synchronize(bb_ctx *ctx) {
     if (!ctx) return BB_ERR_ARG;
     BB_CUDA(ctx, cudaSetDevice(ctx->device));
-    BB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    for (bb_ctx *kid : ctx->kids) BB_CUDA(ctx, cudaStreamSynchronize(kid->stream));
-    return BB_OK;
-}
-
-static int w_last_run_ms(bb_ctx *ctx, float *total_ms, float *stage_ms) {
-    if (!ctx) return BB_ERR_ARG;
-    if (!ctx->ran) return set_err(ctx, BB_ERR_STATE, "no run to time");
-    BB_CUDA(ctx, cudaSetDevice(ctx->device));
-    BB_CUDA(ctx, cudaEventSynchronize(ctx->ev[BB_N_STAGES - 1]));
-    for (int i = 0; i < BB_N_STAGES - 1; i++)
-        BB_CUDA(ctx, cudaEventElapsedTime(&ctx->stage_ms[i], ctx->ev[i], ctx->ev[i + 1]));
-    BB_CUDA(ctx, cudaEventElapsedTime(&ctx->stage_ms[BB_N_STAGES - 1], ctx->ev[0], ctx->ev[BB_N_STAGES - 1]));
-    if (total_ms) *total_ms = ctx->stage_ms[BB_N_STAGES - 1];
-    if (stage_ms) std::memcpy(stage_ms, ctx->stage_ms, sizeof(ctx->stage_ms));
+    for (const auto &w : ctx->workers) BB_CUDA(ctx, cudaStreamSynchronize(w->stream));
     return BB_OK;
 }
 
 // Enqueues the device-to-host copies of a finished (or at least scanned) worker's packed block on its stream.
-static int w_copy_out(bb_ctx *ctx, int64_t base, uint8_t *seq_out, uint8_t *qual_out) {
-    BB_CUDA(ctx, cudaSetDevice(ctx->device));
-    const int64_t total = ctx->h_info->scan.out_total;
+static int w_copy_out(Worker &w, int64_t base, uint8_t *seq_out, uint8_t *qual_out) {
+    BB_CUDA(&w, cudaSetDevice(w.ctx->device));
+    const int64_t total = w.h_info->scan.out_total;
     if (total > 0) {
-        if (!seq_out || !qual_out) return set_err(ctx, BB_ERR_ARG, "null output buffers");
-        BB_CUDA(ctx, cudaMemcpyAsync(seq_out + base, ctx->d_out_seq.p, (size_t)total, cudaMemcpyDeviceToHost, ctx->stream));
-        BB_CUDA(ctx, cudaMemcpyAsync(qual_out + base, ctx->d_out_qual.p, (size_t)total, cudaMemcpyDeviceToHost, ctx->stream));
+        if (!seq_out || !qual_out) return set_err(&w, BB_ERR_ARG, "null output buffers");
+        BB_CUDA(&w, cudaMemcpyAsync(seq_out + base, w.d_out_seq.p, (size_t)total, cudaMemcpyDeviceToHost, w.stream));
+        BB_CUDA(&w, cudaMemcpyAsync(qual_out + base, w.d_out_qual.p, (size_t)total, cudaMemcpyDeviceToHost, w.stream));
     }
     return BB_OK;
 }
 
 // results[pos[i]] describes the worker's i-th read, its out_off shifted by `base` (from the records w_finish fetched).
-static int w_results(bb_ctx *ctx, bb_read_result *results, const int32_t *pos, int64_t base) {
-    const int n = ctx->n_reads;
+static int w_results(Worker &w, bb_read_result *results, const int32_t *pos, int64_t base) {
+    const int n = w.n_reads;
     int bad = 0, bad_read = -1;
     for (int r = 0; r < n; r++) {
-        const BBReadDev &rd = ctx->h_res[(size_t)r];
+        const BBReadDev &rd = w.h_res[(size_t)r];
         if (results) {
             bb_read_result &o = results[pos ? pos[r] : r];
-            o.out_off = base + rd.out_off; o.out_len = rd.out_len; o.frag_len = ctx->h_inlen[(size_t)r];
+            o.out_off = base + rd.out_off; o.out_len = rd.out_len; o.frag_len = w.h_inlen[(size_t)r];
             o.matches = rd.matches; o.columns = rd.seq_len + rd.dels; o.loop_count = rd.loop_count;
             o.change_count = rd.change_count; o.n_alignments = rd.n_align; o.flags = rd.flags;
             o.loop_kcycles = rd.kc_loop; o.align_kcycles = rd.kc_align;
@@ -1015,34 +1038,27 @@ static int w_results(bb_ctx *ctx, bb_read_result *results, const int32_t *pos, i
     if (bad) {
         char msg[160];
         std::snprintf(msg, sizeof(msg), "device invariant violated: read %d flags 0x%x", pos ? pos[bad_read] : bad_read, bad);
-        return set_err(ctx, BB_ERR_INTERNAL, msg);
+        return set_err(&w, BB_ERR_INTERNAL, msg);
     }
     return BB_OK;
 }
 
 // ---- batch entry points: deal the reads out over the workers ---------------------------------------------
-static bb_ctx *worker_of(bb_ctx *ctx, int w) { return w == 0 ? ctx : ctx->kids[(size_t)w - 1]; }
-
 extern "C" int bb_batch_upload(bb_ctx *ctx, int32_t n_reads, const uint64_t *read_index, const int32_t *seg_off,
                                const bb_segment *segs, const uint8_t *literal_pool, int64_t literal_len,
                                const double *target_identity) {
     if (!ctx) return BB_ERR_ARG;
     if (n_reads <= 0 || !read_index || !seg_off || !segs || !target_identity || literal_len < 0)
         return set_err(ctx, BB_ERR_ARG, "bb_batch_upload: bad arguments");
-    const int n_workers = 1 + (int)ctx->kids.size();
-    ctx->n_split = (n_workers > 1 && n_reads >= 64 * n_workers) ? n_workers : 1;
-    if (ctx->n_split == 1) {
-        ctx->is_head = false;
-        ctx->grid_div = 1;
-        return w_batch_upload(ctx, n_reads, read_index, seg_off, segs, literal_pool, literal_len, target_identity);
-    }
+    if (!ctx->have_em || !ctx->have_qm) return set_err(ctx, BB_ERR_STATE, "upload the error and qscore models first");
+    std::vector<int64_t> len;
+    if (const int rc = check_batch(ctx, n_reads, seg_off, segs, literal_len, len)) return rc;
+    const int n_workers = (int)ctx->workers.size();
+    const int S = ctx->n_split = (n_workers > 1 && n_reads >= 64 * n_workers) ? n_workers : 1;
+    ctx->w0().is_head = false;
+    if (S == 1)
+        return each_worker(ctx, [&](Worker &w, int) -> int { return w_batch_upload(w, n_reads, read_index, seg_off, segs, literal_pool, literal_len, target_identity); });
     // deal the reads out longest first, so that every worker sees the same length distribution
-    const int S = ctx->n_split;
-    std::vector<int64_t> len((size_t)n_reads, 0);
-    for (int32_t r = 0; r < n_reads; r++) {
-        if (seg_off[r + 1] < seg_off[r]) return set_err(ctx, BB_ERR_ARG, "seg_off must be non-decreasing");
-        for (int32_t x = seg_off[r]; x < seg_off[r + 1]; x++) len[(size_t)r] += segs[x].len;
-    }
     std::vector<int32_t> order((size_t)n_reads);
     std::iota(order.begin(), order.end(), 0);
     std::stable_sort(order.begin(), order.end(), [&](int32_t x, int32_t y) { return len[(size_t)x] > len[(size_t)y]; });
@@ -1051,7 +1067,7 @@ extern "C" int bb_batch_upload(bb_ctx *ctx, int32_t n_reads, const uint64_t *rea
     // small HEAD batch of the longest reads: its error loop is short, so their alignment starts early and overlaps the
     // other workers' error loops instead of trailing the step.  The other workers share the rest evenly.
     int32_t n_head = 0;
-    if (S >= 3 && ctx->head_worker) {
+    if (S >= 3 && ctx->knobs.head_worker) {
         int64_t total = 0, hb = 0;
         for (int32_t r = 0; r < n_reads; r++) total += len[(size_t)r];
         const int64_t longest = len[(size_t)order[0]];
@@ -1062,14 +1078,9 @@ extern "C" int bb_batch_upload(bb_ctx *ctx, int32_t n_reads, const uint64_t *rea
         }
         if (n_head < 16) { ctx->part[0].clear(); n_head = 0; }
     }
-    ctx->is_head = n_head > 0;
-    {   // share of the SMs each worker's persistent kernels ask for (BADREAD_B200_GRID_DIV overrides; 1 = all of them)
-        int div = ctx->grid_div_env > 0 ? ctx->grid_div_env : 1;
-        for (int w = 0; w < S; w++) worker_of(ctx, w)->grid_div = div;
-    }
+    ctx->w0().is_head = n_head > 0;
     if (n_head > 0) for (int32_t i = n_head; i < n_reads; i++) ctx->part[(size_t)(1 + (i - n_head) % (S - 1))].push_back(order[(size_t)i]);
     else for (int32_t i = 0; i < n_reads; i++) ctx->part[(size_t)(i % S)].push_back(order[(size_t)i]);
-    constexpr int kBadLiteral = 1 << 20;  // not a bb_status value
     std::vector<int> rcs((size_t)S, 0);
     std::vector<std::thread> threads;
     auto upload_part = [&](int w) {
@@ -1083,7 +1094,6 @@ extern "C" int bb_batch_upload(bb_ctx *ctx, int32_t n_reads, const uint64_t *rea
             for (int32_t x = seg_off[r]; x < seg_off[r + 1]; x++) {
                 bb_segment g = segs[x];
                 if (g.kind == BB_SEG_LITERAL) {
-                    if (g.len < 0 || g.src < 0 || g.src + g.len > literal_len) { rcs[(size_t)w] = kBadLiteral; return; }
                     const int64_t at = (int64_t)lit.size();
                     lit.insert(lit.end(), literal_pool + g.src, literal_pool + g.src + g.len);
                     g.src = at;
@@ -1092,36 +1102,29 @@ extern "C" int bb_batch_upload(bb_ctx *ctx, int32_t n_reads, const uint64_t *rea
             }
             soff.push_back((int32_t)sg.size());
         }
-        rcs[(size_t)w] = w_batch_upload(worker_of(ctx, w), (int32_t)mine.size(), ridx.data(), soff.data(), sg.data(),
+        rcs[(size_t)w] = w_batch_upload(*ctx->workers[(size_t)w], (int32_t)mine.size(), ridx.data(), soff.data(), sg.data(),
                                         lit.data(), (int64_t)lit.size(), ident.data());
     };
     for (int w = 1; w < S; w++) threads.emplace_back(upload_part, w);
     upload_part(0);
     for (auto &t : threads) t.join();
-    for (int w = 0; w < S; w++) {
-        if (rcs[(size_t)w] == kBadLiteral) return set_err(ctx, BB_ERR_ARG, "literal segment out of range");
-        if (rcs[(size_t)w]) return w == 0 ? rcs[0] : set_err(ctx, rcs[(size_t)w], worker_of(ctx, w)->err);
-    }
-    return BB_OK;
+    return each_worker(ctx, [&](Worker &, int w) -> int { return rcs[(size_t)w]; });
 }
 
 // Asynchronous: the kernel chains of all workers are enqueued from this thread and overlap on the device.
 extern "C" int bb_batch_run(bb_ctx *ctx) {
     if (!ctx) return BB_ERR_ARG;
-    const int S = ctx->n_split;
-    for (int w = 0; w < S; w++) {
-        bb_ctx *wk = worker_of(ctx, w);
-        wk->reran = false; wk->n_reruns = 0; wk->rerun_reasons = 0;
-    }
     BB_CUDA(ctx, cudaSetDevice(ctx->device));
-    BB_CUDA(ctx, cudaEventRecord(ctx->ev_t0, ctx->stream));
-    for (int w = 1; w < S; w++) BB_CUDA(ctx, cudaStreamWaitEvent(worker_of(ctx, w)->stream, ctx->ev_t0, 0));
-    for (int w = 0; w < S; w++) {
-        const int rc = w_enqueue(worker_of(ctx, w));
-        if (rc) return w == 0 ? rc : set_err(ctx, rc, worker_of(ctx, w)->err);
-    }
-    for (int w = 1; w < S; w++) BB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, worker_of(ctx, w)->ev[BB_N_STAGES - 1], 0));
-    BB_CUDA(ctx, cudaEventRecord(ctx->ev_t1, ctx->stream));
+    const cudaStream_t st0 = ctx->w0().stream;
+    BB_CUDA(ctx, cudaEventRecord(ctx->ev_t0, st0));
+    int rc = each_worker(ctx, [&](Worker &w, int i) -> int {
+        w.reran = false; w.n_reruns = 0; w.rerun_reasons = 0;
+        if (i > 0) BB_CUDA(&w, cudaStreamWaitEvent(w.stream, ctx->ev_t0, 0));
+        return w_enqueue(w);
+    });
+    if (rc) return rc;
+    for (int w = 1; w < ctx->n_split; w++) BB_CUDA(ctx, cudaStreamWaitEvent(st0, ctx->workers[(size_t)w]->ev[BB_N_STAGES - 1], 0));
+    BB_CUDA(ctx, cudaEventRecord(ctx->ev_t1, st0));
     return BB_OK;
 }
 
@@ -1130,9 +1133,8 @@ extern "C" int bb_last_run_retries(const bb_ctx *ctx, int32_t *n_reruns, uint32_
     int32_t total = 0;
     uint32_t bits = 0;
     for (int w = 0; w < ctx->n_split; w++) {
-        const bb_ctx *wk = w == 0 ? ctx : ctx->kids[(size_t)w - 1];
-        total += wk->n_reruns;
-        bits |= wk->rerun_reasons;
+        total += ctx->workers[(size_t)w]->n_reruns;
+        bits |= ctx->workers[(size_t)w]->rerun_reasons;
     }
     if (n_reruns) *n_reruns = total;
     if (reasons) *reasons = bits;
@@ -1142,15 +1144,15 @@ extern "C" int bb_last_run_retries(const bb_ctx *ctx, int32_t *n_reruns, uint32_
 // Task counts of the last run of every worker (see include/badread_b200.h); read from the counters w_finish fetched.
 extern "C" int bb_last_run_work(const bb_ctx *ctx, int64_t *work, int64_t *level_nodes, int32_t level_cap, int32_t *n_levels) {
     if (!ctx) return BB_ERR_ARG;
-    if (level_cap < 0 || (level_cap > 0 && !level_nodes)) return set_err(const_cast<bb_ctx *>(ctx), BB_ERR_ARG, "bb_last_run_work: bad arguments");
+    bb_ctx *mctx = const_cast<bb_ctx *>(ctx);  // for the error message
+    if (level_cap < 0 || (level_cap > 0 && !level_nodes)) return set_err(mctx, BB_ERR_ARG, "bb_last_run_work: bad arguments");
     int64_t w[BB_WORK_SLOTS] = {};
     if (level_nodes) std::fill(level_nodes, level_nodes + (size_t)level_cap * BBQ_NODE_CLASSES, 0);
     int levels = 0;
-    for (int x = 0; x < ctx->n_split; x++) {
-        const bb_ctx *wk = x == 0 ? ctx : ctx->kids[(size_t)x - 1];
-        if (!wk->finished) return set_err(const_cast<bb_ctx *>(ctx), BB_ERR_STATE, "bb_last_run_work: fetch the batch first");
-        const bb_ctx::RunInfo &info = *wk->h_info;
-        for (int r = 0; r < wk->n_rounds; r++) {  // each kernel passes what it cannot take on to the next
+    const int rc = each_worker(mctx, [&](Worker &wk, int) -> int {
+        if (!wk.finished) return set_err(&wk, BB_ERR_STATE, "bb_last_run_work: fetch the batch first");
+        const Worker::RunInfo &info = *wk.h_info;
+        for (int r = 0; r < wk.n_rounds; r++) {  // each kernel passes what it cannot take on to the next
             const int *c = info.counters + BB_ROUND_BASE(r);
             w[BB_WORK_WINDOW_LANE4] += c[BBC_NTASKS] - c[BBC_FB1];
             w[BB_WORK_WINDOW_LANE8] += c[BBC_FB1] - c[BBC_FB2];
@@ -1164,8 +1166,10 @@ extern "C" int bb_last_run_work(const bb_ctx *ctx, int64_t *work, int64_t *level
             for (int l = 0; l < std::min(level_cap, BB_MAX_LEVELS); l++)
                 for (int c = 0; c < BBQ_NODE_CLASSES; c++) level_nodes[(size_t)l * BBQ_NODE_CLASSES + c] += info.levels[s][l][c];
         }
-        levels = std::max(levels, wk->n_levels);
-    }
+        levels = std::max(levels, wk.n_levels);
+        return BB_OK;
+    });
+    if (rc) return rc;
     if (work) std::memcpy(work, w, sizeof(w));
     if (n_levels) *n_levels = levels;
     return BB_OK;
@@ -1176,23 +1180,26 @@ extern "C" int bb_last_run_work(const bb_ctx *ctx, int64_t *work, int64_t *level
 // per-worker stage times, scaled to the whole-batch time.
 extern "C" int bb_last_run_ms(bb_ctx *ctx, float *total_ms, float *stage_ms) {
     if (!ctx) return BB_ERR_ARG;
-    const int S = ctx->n_split;
-    float sum[BB_N_STAGES] = {};
-    for (int w = 0; w < S; w++) {
-        float t = 0.f, st[BB_N_STAGES];
-        const int rc = w_last_run_ms(worker_of(ctx, w), &t, st);
-        if (rc) return w == 0 ? rc : set_err(ctx, rc, worker_of(ctx, w)->err);
-        for (int i = 0; i < BB_N_STAGES; i++) sum[i] += st[i];
-    }
     BB_CUDA(ctx, cudaSetDevice(ctx->device));
+    float sum[BB_N_STAGES] = {};
+    const int rc = each_worker(ctx, [&](Worker &w, int) -> int {
+        if (!w.ran) return set_err(&w, BB_ERR_STATE, "no run to time");
+        BB_CUDA(&w, cudaEventSynchronize(w.ev[BB_N_STAGES - 1]));
+        for (int i = 0; i < BB_N_STAGES; i++) {  // between consecutive events; the last stage is the whole chain
+            const bool all = i == BB_N_STAGES - 1;
+            float t = 0.f;
+            BB_CUDA(&w, cudaEventElapsedTime(&t, w.ev[all ? 0 : i], w.ev[all ? i : i + 1]));
+            sum[i] += t;
+        }
+        return BB_OK;
+    });
+    if (rc) return rc;
     BB_CUDA(ctx, cudaEventSynchronize(ctx->ev_t1));
     float total = 0.f;
     BB_CUDA(ctx, cudaEventElapsedTime(&total, ctx->ev_t0, ctx->ev_t1));
     const float scale = sum[BB_N_STAGES - 1] > 0.f ? total / sum[BB_N_STAGES - 1] : 0.f;
-    for (int i = 0; i < BB_N_STAGES - 1; i++) ctx->stage_ms[i] = sum[i] * scale;
-    ctx->stage_ms[BB_N_STAGES - 1] = total;
     if (total_ms) *total_ms = total;
-    if (stage_ms) std::memcpy(stage_ms, ctx->stage_ms, sizeof(ctx->stage_ms));
+    for (int i = 0; stage_ms && i < BB_N_STAGES; i++) stage_ms[i] = i < BB_N_STAGES - 1 ? sum[i] * scale : total;
     return BB_OK;
 }
 
@@ -1200,26 +1207,25 @@ extern "C" int bb_last_run_ms(bb_ctx *ctx, float *total_ms, float *stage_ms) {
 // first worker's first mark; "begin" is the previous mark on the same worker and stream.
 extern "C" int bb_trace_dump(bb_ctx *ctx, const char *path) {
     if (!ctx || !path) return BB_ERR_ARG;
-    if (!ctx->trace || ctx->marks.empty()) return set_err(ctx, BB_ERR_STATE, "no trace (set BADREAD_B200_TRACE=1 before bb_create)");
+    if (!ctx->knobs.trace || ctx->w0().marks.empty()) return set_err(ctx, BB_ERR_STATE, "no trace (set BADREAD_B200_TRACE=1 before bb_create)");
     BB_CUDA(ctx, cudaSetDevice(ctx->device));
     BB_CUDA(ctx, cudaDeviceSynchronize());
     FILE *f = std::fopen(path, "w");
     if (!f) return set_err(ctx, BB_ERR_ARG, "cannot open trace file");
     std::fprintf(f, "worker,stream,name,begin_ms,end_ms\n");
-    const cudaEvent_t base = ctx->marks[0].ev;
-    const int S = ctx->n_split;
-    for (int w = 0; w < S; w++) {
-        bb_ctx *wk = w == 0 ? ctx : ctx->kids[(size_t)w - 1];
+    const cudaEvent_t base = ctx->w0().marks[0].ev;
+    each_worker(ctx, [&](Worker &wk, int w) -> int {
         float prev[10] = {};
         bool have[10] = {};
-        for (const bb_ctx::Mark &m : wk->marks) {
+        for (const Worker::Mark &m : wk.marks) {
             float t = 0.f;
             if (cudaEventElapsedTime(&t, base, m.ev) != cudaSuccess) continue;
             const float b = have[m.stream] ? prev[m.stream] : (have[0] ? prev[0] : t);
             std::fprintf(f, "%d,%d,%s,%.4f,%.4f\n", w, m.stream, m.name, b, t);
             prev[m.stream] = t; have[m.stream] = true;
         }
-    }
+        return BB_OK;
+    });
     std::fclose(f);
     return BB_OK;
 }
@@ -1228,38 +1234,29 @@ extern "C" int bb_trace_dump(bb_ctx *ctx, const char *path) {
 // eager: the copies of a worker were already enqueued behind its kernels with these bases (bb_sequence_batch).
 static int fetch_all(bb_ctx *ctx, bb_read_result *results, uint8_t *seq_out, uint8_t *qual_out, int64_t out_cap,
                      int64_t *out_total, const std::vector<int64_t> *eager_bases) {
-    const int S = ctx->n_split;
-    std::vector<int64_t> base((size_t)S, 0);
+    std::vector<int64_t> base((size_t)ctx->n_split, 0);
     int64_t total = 0;
     bool moved = false;  // a worker's output size changed after the eager copies were placed (it had to run again)
-    for (int w = 0; w < S; w++) {
-        bb_ctx *wk = worker_of(ctx, w);
-        if (!wk->ran) return set_err(ctx, BB_ERR_STATE, "bb_fetch_last_batch: nothing to fetch");
-        const int rc = w_finish(wk);
-        if (rc) return w == 0 ? rc : set_err(ctx, rc, wk->err);
-        if (wk->reran) moved = true;
-        base[(size_t)w] = total;
-        total += wk->out_total;
-    }
-    ctx->part_base = base;
+    int rc = each_worker(ctx, [&](Worker &w, int i) -> int {
+        if (!w.ran) return set_err(&w, BB_ERR_STATE, "bb_fetch_last_batch: nothing to fetch");
+        if (const int rc = w_finish(w)) return rc;
+        if (w.reran) moved = true;
+        base[(size_t)i] = total;
+        total += w.h_info->scan.out_total;
+        return BB_OK;
+    });
+    if (rc) return rc;
     if (out_total) *out_total = total;
     if (out_cap < total) return set_err(ctx, BB_ERR_CAPACITY, "output buffers too small");
     if (total && (!seq_out || !qual_out)) return set_err(ctx, BB_ERR_ARG, "null output buffers");
     const bool have_eager = eager_bases && !moved && *eager_bases == base;
-    if (!have_eager) {
-        for (int w = 0; w < S; w++) {
-            const int rc = w_copy_out(worker_of(ctx, w), base[(size_t)w], seq_out, qual_out);
-            if (rc) return w == 0 ? rc : set_err(ctx, rc, worker_of(ctx, w)->err);
-        }
-    }
-    for (int w = 0; w < S; w++) {
-        bb_ctx *wk = worker_of(ctx, w);
-        BB_CUDA(ctx, cudaSetDevice(wk->device));
-        BB_CUDA(ctx, cudaStreamSynchronize(wk->stream));
-        const int rc = w_results(wk, results, S == 1 ? nullptr : ctx->part[(size_t)w].data(), base[(size_t)w]);
-        if (rc) return w == 0 ? rc : set_err(ctx, rc, wk->err);
-    }
-    return BB_OK;
+    if (!have_eager && (rc = each_worker(ctx, [&](Worker &w, int i) -> int { return w_copy_out(w, base[(size_t)i], seq_out, qual_out); })))
+        return rc;
+    return each_worker(ctx, [&](Worker &w, int i) -> int {
+        BB_CUDA(&w, cudaSetDevice(ctx->device));
+        BB_CUDA(&w, cudaStreamSynchronize(w.stream));
+        return w_results(w, results, ctx->n_split == 1 ? nullptr : ctx->part[(size_t)i].data(), base[(size_t)i]);
+    });
 }
 
 extern "C" int bb_fetch_last_batch(bb_ctx *ctx, bb_read_result *results, uint8_t *seq_out, uint8_t *qual_out,
@@ -1282,35 +1279,35 @@ extern "C" int bb_sequence_batch(bb_ctx *ctx, int32_t n_reads, const uint64_t *r
     int64_t total = 0;
     bool eager = true;
     for (int w = 0; w < S && eager; w++) {
-        bb_ctx *wk = worker_of(ctx, w);
-        BB_CUDA(ctx, cudaSetDevice(wk->device));
-        BB_CUDA(ctx, cudaEventSynchronize(wk->ev_scan));
+        Worker &wk = *ctx->workers[(size_t)w];
+        BB_CUDA(ctx, cudaSetDevice(ctx->device));
+        BB_CUDA(ctx, cudaEventSynchronize(wk.ev_scan));
         base[(size_t)w] = total;
-        total += wk->h_info->scan.out_total;
+        total += wk.h_info->scan.out_total;
         // (a worker with reads that did not fit or did not finish runs again: its size and everything after it moves)
-        if (wk->h_info->scan.n_nospace > 0 || wk->h_info->scan.n_pending > 0 || total > out_cap) { eager = false; break; }
+        if (wk.h_info->scan.n_nospace > 0 || wk.h_info->scan.n_pending > 0 || total > out_cap) { eager = false; break; }
         if ((rc = w_copy_out(wk, base[(size_t)w], seq_out, qual_out))) { eager = false; break; }
     }
     return fetch_all(ctx, results, seq_out, qual_out, out_cap, out_total, eager ? &base : nullptr);
 }
 
-// ---- single-pair entry points ------------------------------------------------------------------------
-static int align_pair_device(bb_ctx *ctx, const uint8_t *q, int n, const uint8_t *t, int m, DevBuf &dq, DevBuf &dt,
-                             DevBuf &dops, DevBuf &ddcnt, DevBuf &dout, int out5[5]) {
+// ---- single-pair entry points (worker 0's stream and scratch) ----------------------------------------------
+static int align_pair_device(bb_ctx *ctx, const uint8_t *q, int n, const uint8_t *t, int m, int out5[5]) {
+    Worker &w = ctx->w0();
     int rc;
-    if ((rc = upload(ctx, dq, q, (size_t)n))) return rc;
-    if ((rc = upload(ctx, dt, t, (size_t)m))) return rc;
-    BB_CUDA(ctx, dops.ensure((size_t)n + 16));
-    BB_CUDA(ctx, ddcnt.ensure(((size_t)n + 16) * sizeof(unsigned int)));
-    BB_CUDA(ctx, dout.ensure(8 * sizeof(int)));
-    if ((rc = ensure_scratch(ctx, std::max(n, m), std::max(n, m), std::max(n, m)))) return rc;
-    BB_CUDA(ctx, cudaMemsetAsync(ddcnt.p, 0, ((size_t)n + 16) * sizeof(unsigned int), ctx->stream));
-    BB_CUDA(ctx, cudaMemsetAsync(dout.p, 0, 8 * sizeof(int), ctx->stream));
-    bbl_align_pair(ctx->stream, dq.as<uint8_t>(), n, dt.as<uint8_t>(), m, std::max(n, m), ctx->pool, dops.as<uint8_t>(),
-                   ddcnt.as<unsigned int>(), dout.as<int>());
-    ctx->launches++;
-    BB_CUDA(ctx, cudaMemcpyAsync(out5, dout.p, 5 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    BB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if ((rc = upload(ctx, w.stream, w.p_q, q, (size_t)n))) return rc;
+    if ((rc = upload(ctx, w.stream, w.p_t, t, (size_t)m))) return rc;
+    BB_CUDA(ctx, w.p_ops.ensure((size_t)n + 16));
+    BB_CUDA(ctx, w.p_dcnt.ensure(((size_t)n + 16) * sizeof(unsigned int)));
+    BB_CUDA(ctx, w.p_out.ensure(8 * sizeof(int)));
+    if ((rc = ensure_scratch(w, std::max(n, m), std::max(n, m), std::max(n, m)))) return set_err(ctx, rc, w.err);
+    BB_CUDA(ctx, cudaMemsetAsync(w.p_dcnt.p, 0, ((size_t)n + 16) * sizeof(unsigned int), w.stream));
+    BB_CUDA(ctx, cudaMemsetAsync(w.p_out.p, 0, 8 * sizeof(int), w.stream));
+    bbl_align_pair(w.stream, w.p_q.as<uint8_t>(), n, w.p_t.as<uint8_t>(), m, std::max(n, m), w.pool, w.p_ops.as<uint8_t>(),
+                   w.p_dcnt.as<unsigned int>(), w.p_out.as<int>());
+    w.launches++;
+    BB_CUDA(ctx, cudaMemcpyAsync(out5, w.p_out.p, 5 * sizeof(int), cudaMemcpyDeviceToHost, w.stream));
+    BB_CUDA(ctx, cudaStreamSynchronize(w.stream));
     if (out5[4]) {
         char msg[96];
         std::snprintf(msg, sizeof(msg), "aligner invariant violated (code 0x%x)", out5[4]);
@@ -1324,14 +1321,14 @@ extern "C" int bb_align_path(bb_ctx *ctx, const uint8_t *query, int32_t q_len, c
     if (!ctx) return BB_ERR_ARG;
     if (!query || !target || q_len <= 0 || t_len <= 0) return set_err(ctx, BB_ERR_ARG, "bb_align_path: empty sequence");
     BB_CUDA(ctx, cudaSetDevice(ctx->device));
-    DevBuf &dq = ctx->p_q, &dt = ctx->p_t, &dops = ctx->p_ops, &ddcnt = ctx->p_dcnt, &dout = ctx->p_out;
+    const Worker &w = ctx->w0();
     int out5[5] = {0, 0, 0, 0, 0};
-    int rc = align_pair_device(ctx, query, q_len, target, t_len, dq, dt, dops, ddcnt, dout, out5);
+    int rc = align_pair_device(ctx, query, q_len, target, t_len, out5);
     std::vector<uint8_t> ops((size_t)q_len);
     std::vector<unsigned int> dcnt((size_t)q_len);
     if (rc == BB_OK) {
-        cudaMemcpy(ops.data(), dops.p, (size_t)q_len, cudaMemcpyDeviceToHost);
-        cudaMemcpy(dcnt.data(), ddcnt.p, (size_t)q_len * sizeof(unsigned int), cudaMemcpyDeviceToHost);
+        cudaMemcpy(ops.data(), w.p_ops.p, (size_t)q_len, cudaMemcpyDeviceToHost);
+        cudaMemcpy(dcnt.data(), w.p_dcnt.p, (size_t)q_len * sizeof(unsigned int), cudaMemcpyDeviceToHost);
     }
     if (rc) return rc;
     const int64_t total = (int64_t)q_len + out5[1];
@@ -1339,13 +1336,13 @@ extern "C" int bb_align_path(bb_ctx *ctx, const uint8_t *query, int32_t q_len, c
     if (distance) *distance = out5[2];
     if (total > ops_cap) return set_err(ctx, BB_ERR_CAPACITY, "ops buffer too small");
     static const char sym[3] = {'=', 'X', 'I'};
-    int64_t w = 0;
-    for (int x = 0; x < out5[3]; x++) ops_out[w++] = 'D';
+    int64_t x = 0;
+    for (int i = 0; i < out5[3]; i++) ops_out[x++] = 'D';
     for (int i = 0; i < q_len; i++) {
-        ops_out[w++] = (uint8_t)sym[ops[(size_t)i] < 3 ? ops[(size_t)i] : 0];
-        for (unsigned int x = 0; x < dcnt[(size_t)i]; x++) ops_out[w++] = 'D';
+        ops_out[x++] = (uint8_t)sym[ops[(size_t)i] < 3 ? ops[(size_t)i] : 0];
+        for (unsigned int d = 0; d < dcnt[(size_t)i]; d++) ops_out[x++] = 'D';
     }
-    if (w != total) return set_err(ctx, BB_ERR_INTERNAL, "column count mismatch");
+    if (x != total) return set_err(ctx, BB_ERR_INTERNAL, "column count mismatch");
     return BB_OK;
 }
 
@@ -1356,19 +1353,19 @@ extern "C" int bb_get_qscores(bb_ctx *ctx, uint64_t read_index, const uint8_t *s
     if (!seq || !frag || seq_len <= 0 || frag_len <= 0 || !qual_out) return set_err(ctx, BB_ERR_ARG, "bb_get_qscores: bad arguments");
     if (!ctx->have_qm) return set_err(ctx, BB_ERR_STATE, "upload the qscore model first");
     BB_CUDA(ctx, cudaSetDevice(ctx->device));
-    DevBuf &dq = ctx->p_q, &dt = ctx->p_t, &dops = ctx->p_ops, &ddcnt = ctx->p_dcnt, &dout = ctx->p_out, &dqual = ctx->p_qual;
+    Worker &w = ctx->w0();
     int out5[5] = {0, 0, 0, 0, 0};
-    int rc = align_pair_device(ctx, seq, seq_len, frag, frag_len, dq, dt, dops, ddcnt, dout, out5);
+    int rc = align_pair_device(ctx, seq, seq_len, frag, frag_len, out5);
     if (rc == BB_OK) {
-        cudaError_t e = dqual.ensure((size_t)seq_len + 16);
+        cudaError_t e = w.p_qual.ensure((size_t)seq_len + 16);
         if (e != cudaSuccess) rc = set_err(ctx, BB_ERR_CUDA, cudaGetErrorString(e));
     }
     if (rc == BB_OK) {
-        bb_k_qscores_pair<<<(seq_len + 255) / 256, 256, 0, ctx->stream>>>(dops.as<uint8_t>(), ddcnt.as<unsigned int>(), seq_len,
-                                                                            ctx->qm, ctx->seed, read_index, dqual.as<uint8_t>());
-        ctx->launches++;
-        cudaMemcpyAsync(qual_out, dqual.p, (size_t)seq_len, cudaMemcpyDeviceToHost, ctx->stream);
-        cudaError_t e = cudaStreamSynchronize(ctx->stream);
+        bb_k_qscores_pair<<<(seq_len + 255) / 256, 256, 0, w.stream>>>(w.p_ops.as<uint8_t>(), w.p_dcnt.as<unsigned int>(), seq_len,
+                                                                        ctx->qm, ctx->seed, read_index, w.p_qual.as<uint8_t>());
+        w.launches++;
+        cudaMemcpyAsync(qual_out, w.p_qual.p, (size_t)seq_len, cudaMemcpyDeviceToHost, w.stream);
+        cudaError_t e = cudaStreamSynchronize(w.stream);
         if (e != cudaSuccess) rc = set_err(ctx, BB_ERR_CUDA, cudaGetErrorString(e));
     }
     if (rc) return rc;
@@ -1494,12 +1491,12 @@ extern "C" int bb_allreduce_bases(bb_ctx *ctx, int64_t local, int64_t *total) {
     BB_CUDA(ctx, cudaSetDevice(ctx->device));
     long long *d = ctx->d_red.as<long long>();
     const long long v = local;
-    BB_CUDA(ctx, cudaMemcpyAsync(d, &v, sizeof(v), cudaMemcpyHostToDevice, ctx->stream));
-    const int rc = nccl().AllReduce(d, d + 1, 1, kNcclInt64, kNcclSum, ctx->nccl_comm, ctx->stream);
+    BB_CUDA(ctx, cudaMemcpyAsync(d, &v, sizeof(v), cudaMemcpyHostToDevice, ctx->w0().stream));
+    const int rc = nccl().AllReduce(d, d + 1, 1, kNcclInt64, kNcclSum, ctx->nccl_comm, ctx->w0().stream);
     if (rc) return nccl_err(ctx, "ncclAllReduce", rc);
     long long out = 0;
-    BB_CUDA(ctx, cudaMemcpyAsync(&out, d + 1, sizeof(out), cudaMemcpyDeviceToHost, ctx->stream));
-    BB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    BB_CUDA(ctx, cudaMemcpyAsync(&out, d + 1, sizeof(out), cudaMemcpyDeviceToHost, ctx->w0().stream));
+    BB_CUDA(ctx, cudaStreamSynchronize(ctx->w0().stream));
     *total = out;
     return BB_OK;
 }
@@ -1512,22 +1509,22 @@ extern "C" int bb_allreduce_bases_all(bb_ctx **ctxs, int n, const int64_t *local
     for (int i = 0; i < n; i++) {
         BB_CUDA(ctxs[i], cudaSetDevice(ctxs[i]->device));
         const long long v = local[i];
-        BB_CUDA(ctxs[i], cudaMemcpyAsync(ctxs[i]->d_red.p, &v, sizeof(v), cudaMemcpyHostToDevice, ctxs[i]->stream));
-        BB_CUDA(ctxs[i], cudaStreamSynchronize(ctxs[i]->stream));  // `v` leaves scope
+        BB_CUDA(ctxs[i], cudaMemcpyAsync(ctxs[i]->d_red.p, &v, sizeof(v), cudaMemcpyHostToDevice, ctxs[i]->w0().stream));
+        BB_CUDA(ctxs[i], cudaStreamSynchronize(ctxs[i]->w0().stream));  // `v` leaves scope
     }
     int rc = nccl().GroupStart();
     for (int i = 0; i < n && !rc; i++) {
         long long *d = ctxs[i]->d_red.as<long long>();
-        rc = nccl().AllReduce(d, d + 1, 1, kNcclInt64, kNcclSum, ctxs[i]->nccl_comm, ctxs[i]->stream);
+        rc = nccl().AllReduce(d, d + 1, 1, kNcclInt64, kNcclSum, ctxs[i]->nccl_comm, ctxs[i]->w0().stream);
     }
     const int rc2 = nccl().GroupEnd();
     if (rc || rc2) return nccl_err(ctxs[0], "ncclAllReduce (group)", rc ? rc : rc2);
     long long out = 0;
     BB_CUDA(ctxs[0], cudaSetDevice(ctxs[0]->device));
-    BB_CUDA(ctxs[0], cudaMemcpyAsync(&out, ctxs[0]->d_red.as<long long>() + 1, sizeof(out), cudaMemcpyDeviceToHost, ctxs[0]->stream));
+    BB_CUDA(ctxs[0], cudaMemcpyAsync(&out, ctxs[0]->d_red.as<long long>() + 1, sizeof(out), cudaMemcpyDeviceToHost, ctxs[0]->w0().stream));
     for (int i = 0; i < n; i++) {
         BB_CUDA(ctxs[i], cudaSetDevice(ctxs[i]->device));
-        BB_CUDA(ctxs[i], cudaStreamSynchronize(ctxs[i]->stream));
+        BB_CUDA(ctxs[i], cudaStreamSynchronize(ctxs[i]->w0().stream));
     }
     *total = out;
     return BB_OK;
