@@ -118,6 +118,8 @@ def simulate_subparser(subparsers):
     b200_args.add_argument('--gpus', type=int, default=1, help='GPUs to shard reads over (default: %(default)s)')
     b200_args.add_argument('--batch_reads', type=int, default=16384,
                            help='Reads per GPU per batch (default: %(default)s)')
+    b200_args.add_argument('--gzip', action='store_true',
+                           help='Write the FASTQ as BGZF (gzip-compatible), compressed on the GPUs')
     group.add_argument('--version', action='version', version='Badread v' + __version__)
 
 

@@ -25,6 +25,7 @@ BB_RERUN_ROUNDS, BB_RERUN_SLACK, BB_RERUN_LEVELS, BB_RERUN_QUEUES, BB_RERUN_SCRA
 WORK_SLOTS = ('window_lane4', 'window_lane8', 'window_warp', 'leaf_lane', 'leaf_warp', 'root_leaf_lane', 'root_leaf_warp')
 NODE_CLASSES = ('lane8', 'lean1', 'lean2', 'lean4', 'wide')
 BB_MAX_LEVELS = 48
+BB_BGZF_CHUNK = 65280   # input bytes per BGZF member (bb_bgzf_compress)
 
 
 class Segment(ctypes.Structure):
@@ -130,6 +131,8 @@ def lib():
         'bb_count_cigar_qscores': (c.c_int, [c.c_int, c.c_int, c.c_int, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, i64, vp, vp, vp,
                                              P(i64), vp, i64, vp, vp, vp, P(i64)]),
         'bb_model_error': (c.c_char_p, []),
+        'bb_bgzf_bound': (i64, [i64]),
+        'bb_bgzf_compress': (c.c_int, [vp, vp, i64, c.c_int, c.c_int, vp, i64, P(i64), P(i64)]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(L, name)
@@ -147,4 +150,5 @@ EXPORTED_SYMBOLS = ['bb_create', 'bb_destroy', 'bb_last_error', 'bb_version', 'b
                     'bb_host_align_kmers', 'bb_host_align_path', 'bb_nccl_available', 'bb_comm_unique_id', 'bb_comm_init_rank',
                     'bb_comm_init_all', 'bb_allreduce_bases', 'bb_allreduce_bases_all', 'bb_planner_create', 'bb_planner_destroy',
                     'bb_planner_plan', 'bb_planner_view', 'bb_planner_error', 'bb_fastq_format', 'bb_fastq_format_sharded',
-                    'bb_count_kmer_alternatives', 'bb_count_kmer_alternatives_wide', 'bb_count_cigar_qscores', 'bb_model_error']
+                    'bb_count_kmer_alternatives', 'bb_count_kmer_alternatives_wide', 'bb_count_cigar_qscores', 'bb_model_error',
+                    'bb_bgzf_bound', 'bb_bgzf_compress']

@@ -1,0 +1,94 @@
+"""
+BGZF output of `simulate --gzip`: FASTQ records compressed on the GPUs (Engine.bgzf_compress, csrc/bb_bgzf.cuh) and
+written as BGZF (SAM specification §4.1), which gzip, zlib and htslib read.
+
+Members hold BGZF_CHUNK bytes at fixed offsets of the whole FASTQ stream: the writer carries the tail of every buffer
+into the next one, so the compressed bytes depend neither on the batch size nor on the number of GPUs.
+"""
+import threading
+
+import numpy as np
+
+from ._lib import BB_BGZF_CHUNK as BGZF_CHUNK
+
+# the empty member that ends a BGZF file (SAM specification §4.1.2)
+EOF_MEMBER = bytes.fromhex('1f8b08040000000000ff0600424302001b0003000000000000000000')
+
+
+def _newlines(buf):
+    return int(np.count_nonzero(np.frombuffer(buf, dtype=np.uint8) == 10))
+
+
+class BGZFWriter(object):
+    """Compresses whole FASTQ records with `engines` and writes the members to the binary stream `out` in stream order.
+    With several engines the whole chunks of a buffer are dealt out over them in contiguous runs, one host thread each."""
+
+    def __init__(self, engines, out):
+        self.engines = list(engines)
+        self.out = out
+        self.tail = b''        # input after the last whole chunk
+        self.tail_mod4 = 0     # index mod 4 of the FASTQ line the tail's first byte belongs to
+
+    def write(self, records):
+        """records: a bytes-like object of whole FASTQ records (it starts with a header line and ends with the newline
+        of a quality line)."""
+        data = memoryview(records).cast('B')
+        if len(self.tail) + len(data) < BGZF_CHUNK:
+            self.tail += bytes(data)
+            return
+        mod4 = 0
+        if self.tail:   # the chunk that spans the previous buffer's tail and this buffer's head
+            need = BGZF_CHUNK - len(self.tail)
+            members, _ = self.engines[0].bgzf_compress(self.tail + bytes(data[:need]), self.tail_mod4, final=False)
+            self.out.write(members)
+            mod4 = _newlines(data[:need]) & 3
+            data = data[need:]
+        n_chunks = len(data) // BGZF_CHUNK
+        parts = self._parts(data, n_chunks, mod4)
+        results = [None] * len(parts)
+        errors = [None] * len(parts)
+
+        def work(k):
+            try:
+                results[k] = self.engines[k].bgzf_compress(parts[k][0], parts[k][1], final=False)[0]
+            except BaseException as e:   # re-raised on the caller's thread
+                errors[k] = e
+
+        if len(parts) == 1:
+            work(0)
+        else:
+            threads = [threading.Thread(target=work, args=(k,)) for k in range(len(parts))]
+            for t in threads:
+                t.start()
+            for t in threads:
+                t.join()
+        for e in errors:
+            if e is not None:
+                raise e
+        for members in results:
+            self.out.write(members)
+        self.tail = bytes(data[n_chunks * BGZF_CHUNK:])
+        self.tail_mod4 = -_newlines(self.tail) & 3   # the records end with a quality line: line index 0 mod 4 follows
+
+    def _parts(self, data, n_chunks, mod4):
+        """The whole chunks of data as [(slice, line index mod 4 at its start)], one contiguous run per engine."""
+        n_parts = max(1, min(len(self.engines), n_chunks))
+        per = -(-n_chunks // n_parts) * BGZF_CHUNK
+        bounds = [min(k * per, n_chunks * BGZF_CHUNK) for k in range(n_parts + 1)]
+        lines = [0] * n_parts
+        if n_parts > 1:   # newlines before each run, counted side by side
+            counters = [threading.Thread(target=lambda k=k: lines.__setitem__(k + 1, _newlines(data[bounds[k]:bounds[k + 1]])))
+                        for k in range(n_parts - 1)]
+            for t in counters:
+                t.start()
+            for t in counters:
+                t.join()
+        return [(data[bounds[k]:bounds[k + 1]], (mod4 + sum(lines[:k + 1])) & 3) for k in range(n_parts)]
+
+    def close(self):
+        """Compresses the tail and ends the file with the end-of-file member."""
+        if self.tail:
+            members, _ = self.engines[0].bgzf_compress(self.tail, self.tail_mod4, final=True)
+            self.out.write(members)
+            self.tail = b''
+        self.out.write(EOF_MEMBER)

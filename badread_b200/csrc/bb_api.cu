@@ -211,8 +211,17 @@ struct bb_ctx {
     void *nccl_comm = nullptr;   // ncclComm_t of this context's device (bb_comm_init_rank / bb_comm_init_all)
     DevBuf d_red;                // two int64: send, receive of bb_allreduce_bases
 
+    // BGZF compressor (bb_bgzf_compress): a stream and scratch of its own, so that a call leaves the workers alone
+    cudaStream_t bgzf_stream = nullptr;
+    int64_t *h_bgzf = nullptr;   // pinned: line_pref[n_chunks] and offsets[n_chunks] of the last pass
+    DevBuf bgzf_in, bgzf_slots, bgzf_lines, bgzf_sizes, bgzf_pref, bgzf_off, bgzf_out;
+
     Worker &w0() { return *workers[0]; }
-    ~bb_ctx() { for (cudaEvent_t e : {ev_t0, ev_t1}) if (e) cudaEventDestroy(e); }
+    ~bb_ctx() {
+        for (cudaEvent_t e : {ev_t0, ev_t1}) if (e) cudaEventDestroy(e);
+        if (bgzf_stream) cudaStreamDestroy(bgzf_stream);
+        if (h_bgzf) cudaFreeHost(h_bgzf);
+    }
 };
 
 // Records "the work enqueued on `st` up to here is done" under `name` (tracing only).
@@ -340,6 +349,7 @@ extern "C" int bb_create(bb_ctx **out, int device, uint64_t seed) {
     if (e == cudaSuccess) e = bbl_node_quad_init();
     if (e == cudaSuccess) e = bbl_window_lane_init();
     if (e == cudaSuccess) e = bbl_leaf_lane_init();
+    if (e == cudaSuccess) e = bbl_bgzf_init();
     if (e != cudaSuccess) { g_create_error = cudaGetErrorString(e); return BB_ERR_CUDA; }
     // 2 workers on H100 (132 SMs, 80 GB): as fast as 3 and 12 % faster than 4 on config 1, and their scratch (lane
     // histories sized by the SM count) leaves room for a second context on the same GPU (~39 GB peak against 66 with 4).
@@ -357,6 +367,7 @@ extern "C" int bb_destroy(bb_ctx *ctx) {
     if (!ctx) return BB_OK;
     cudaSetDevice(ctx->device);  // the frees below act on the current device
     for (const auto &w : ctx->workers) cudaStreamSynchronize(w->stream);
+    if (ctx->bgzf_stream) cudaStreamSynchronize(ctx->bgzf_stream);
     if (ctx->nccl_comm && nccl_destroy) nccl_destroy(ctx->nccl_comm);
     delete ctx;
     return BB_OK;
@@ -1005,6 +1016,69 @@ extern "C" int bb_synchronize(bb_ctx *ctx) {
     if (!ctx) return BB_ERR_ARG;
     BB_CUDA(ctx, cudaSetDevice(ctx->device));
     for (const auto &w : ctx->workers) BB_CUDA(ctx, cudaStreamSynchronize(w->stream));
+    return BB_OK;
+}
+
+// A member holds a chunk and at most 31 bytes more: the gzip header with the BC field (18), a stored block's 5 bytes
+// when the chunk does not code smaller, CRC32 and ISIZE (8).
+extern "C" int64_t bb_bgzf_bound(int64_t n) {
+    return n <= 0 ? 0 : n + (n + BB_BGZF_CHUNK - 1) / BB_BGZF_CHUNK * 31;
+}
+
+// Input passes of at most this many chunks (134 MB) bound the scratch the context keeps after a call to about 450 MB
+// (input, member slots and packed members, each with DevBuf's 1/8 slack).  Fewer chunks per pass leave the compressor
+// few waves to even out its slow chunks: 256 (57 MB of scratch) took 51 ms of kernel time on config 1's FASTQ on an H100
+// against 34 ms with 2048.
+constexpr int64_t kBgzfPassChunks = 2048;
+
+extern "C" int bb_bgzf_compress(bb_ctx *ctx, const uint8_t *in, int64_t n, int line_mod4, int final, uint8_t *out,
+                                int64_t out_cap, int64_t *n_out, int64_t *n_consumed) {
+    if (!ctx || n < 0 || (n && !in) || line_mod4 < 0 || line_mod4 > 3 || out_cap < 0 || !n_out || !n_consumed)
+        return set_err(ctx, BB_ERR_ARG, "bb_bgzf_compress: bad arguments");
+    const int64_t use = final ? n : n / BB_BGZF_CHUNK * BB_BGZF_CHUNK;
+    *n_out = 0;
+    *n_consumed = 0;
+    if (bb_bgzf_bound(use) > out_cap || (use && !out)) {
+        *n_out = bb_bgzf_bound(use);
+        return set_err(ctx, BB_ERR_CAPACITY, "bb_bgzf_compress: out_cap is less than bb_bgzf_bound of the input");
+    }
+    BB_CUDA(ctx, cudaSetDevice(ctx->device));
+    if (!ctx->bgzf_stream) {
+        BB_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->bgzf_stream, cudaStreamNonBlocking));
+        BB_CUDA(ctx, cudaHostAlloc((void **)&ctx->h_bgzf, 2 * sizeof(int64_t), cudaHostAllocPortable));
+    }
+    const cudaStream_t st = ctx->bgzf_stream;
+    int mod4 = line_mod4;
+    int64_t done = 0, written = 0;
+    while (done < use) {
+        const int64_t len = std::min(use - done, kBgzfPassChunks * BB_BGZF_CHUNK);
+        const int nc = (int)((len + BB_BGZF_CHUNK - 1) / BB_BGZF_CHUNK);
+        BB_CUDA(ctx, ctx->bgzf_in.ensure((size_t)len));
+        BB_CUDA(ctx, ctx->bgzf_slots.ensure((size_t)nc * 65536));
+        BB_CUDA(ctx, ctx->bgzf_lines.ensure((size_t)nc * sizeof(int32_t)));
+        BB_CUDA(ctx, ctx->bgzf_sizes.ensure((size_t)nc * sizeof(int32_t)));
+        BB_CUDA(ctx, ctx->bgzf_pref.ensure((size_t)(nc + 1) * sizeof(int64_t)));
+        BB_CUDA(ctx, ctx->bgzf_off.ensure((size_t)(nc + 1) * sizeof(int64_t)));
+        BB_CUDA(ctx, ctx->bgzf_out.ensure((size_t)bb_bgzf_bound(len)));
+        BB_CUDA(ctx, cudaMemcpyAsync(ctx->bgzf_in.p, in + done, (size_t)len, cudaMemcpyHostToDevice, st));
+        bbl_bgzf_pass(st, ctx->bgzf_in.as<uint8_t>(), len, nc, mod4, ctx->bgzf_lines.as<int32_t>(), ctx->bgzf_pref.as<int64_t>(),
+                      ctx->bgzf_slots.as<uint8_t>(), ctx->bgzf_sizes.as<int32_t>(), ctx->bgzf_off.as<int64_t>(),
+                      ctx->bgzf_out.as<uint8_t>());
+        BB_CUDA(ctx, cudaGetLastError());
+        BB_CUDA(ctx, cudaMemcpyAsync(ctx->h_bgzf, ctx->bgzf_pref.as<int64_t>() + nc, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+        BB_CUDA(ctx, cudaMemcpyAsync(ctx->h_bgzf + 1, ctx->bgzf_off.as<int64_t>() + nc, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+        BB_CUDA(ctx, cudaStreamSynchronize(st));
+        const int64_t bytes = ctx->h_bgzf[1];
+        if (bytes <= 0 || bytes > bb_bgzf_bound(len))
+            return set_err(ctx, BB_ERR_INTERNAL, "bb_bgzf_compress: members of " + std::to_string(bytes) + " bytes");
+        BB_CUDA(ctx, cudaMemcpyAsync(out + written, ctx->bgzf_out.p, (size_t)bytes, cudaMemcpyDeviceToHost, st));
+        BB_CUDA(ctx, cudaStreamSynchronize(st));
+        mod4 = (int)(ctx->h_bgzf[0] & 3);
+        written += bytes;
+        done += len;
+    }
+    *n_out = written;
+    *n_consumed = use;
     return BB_OK;
 }
 

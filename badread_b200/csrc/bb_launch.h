@@ -36,3 +36,9 @@ cudaError_t bbl_leaf_lane_init();
 void bbl_leaf_lane(int grid, cudaStream_t st, BBBatchDev B, BBQueues Q, uint32_t *ckpt_pool, int *cursor);
 void bbl_align_pair(cudaStream_t st, const uint8_t *q, int n, const uint8_t *t, int m, int k_upper, BBScratchPool pool,
                     uint8_t *ops, unsigned int *dcnt, int *out5);
+// BGZF (bb_bgzf.cuh): the n_chunks chunks of in[0..n) -> members packed back to back into out, out[offsets[n_chunks]]
+// bytes in all; line_mod4: index mod 4 of the FASTQ line in[0] belongs to; line_pref[n_chunks] = line_mod4 + newlines.
+// Scratch: lines[n_chunks], line_pref and offsets[n_chunks + 1], slots[n_chunks * BGZF_SLOT], sizes[n_chunks].
+cudaError_t bbl_bgzf_init();
+void bbl_bgzf_pass(cudaStream_t st, const uint8_t *in, int64_t n, int n_chunks, int line_mod4, int32_t *lines,
+                   int64_t *line_pref, uint8_t *slots, int32_t *sizes, int64_t *offsets, uint8_t *out);

@@ -131,6 +131,7 @@ class Engine(object):
         self._out_cap = 0
         self._seq_buf = self._qual_buf = None
         self._pinned = []
+        self._bgzf_buf = None
 
     def close(self):
         if getattr(self, '_ctx', None):
@@ -203,7 +204,7 @@ class Engine(object):
             self._out_cap = cap
 
     def _free_out(self):
-        self._seq_buf = self._qual_buf = None
+        self._seq_buf = self._qual_buf = self._bgzf_buf = None
         self._out_cap = 0
         for p in self._pinned:
             self._lib.bb_host_free(p)
@@ -293,6 +294,27 @@ class Engine(object):
                                                self._out_cap, ctypes.byref(total))
         self._check(rc, 'bb_sequence_batch')
         return BatchResult(results, self._seq_buf, self._qual_buf, n), int(total.value)
+
+    # ---- BGZF output
+    def bgzf_compress(self, buf, line_mod4=0, final=False):
+        """BGZF members of FASTQ text on this GPU (bb_bgzf_compress): buf is any bytes-like object, line_mod4 the index
+        mod 4 of the FASTQ line its first byte belongs to.  Without `final` only the whole chunks of _lib.BB_BGZF_CHUNK bytes
+        are compressed.  Returns (members, bytes of buf consumed); members is a uint8 array in page-locked memory that the
+        next call reuses.  The end-of-file member is not included (badread_b200.bgzf.EOF_MEMBER)."""
+        data = np.frombuffer(buf, dtype=np.uint8)
+        need = int(self._lib.bb_bgzf_bound(data.size))
+        if self._bgzf_buf is None or self._bgzf_buf.size < need:
+            cap = max(need + need // 8, 1 << 20)
+            p = ctypes.c_void_p()
+            if self._lib.bb_host_alloc(ctypes.byref(p), cap) != 0:
+                raise EngineError(f'bb_host_alloc({cap}) failed')
+            self._pinned.append(p)
+            self._bgzf_buf = np.ctypeslib.as_array((ctypes.c_uint8 * cap).from_address(p.value))
+        n_out, n_used = ctypes.c_int64(0), ctypes.c_int64(0)
+        rc = self._lib.bb_bgzf_compress(self._ctx, _ptr(data) if data.size else None, data.size, int(line_mod4), int(bool(final)),
+                                        _ptr(self._bgzf_buf), self._bgzf_buf.size, ctypes.byref(n_out), ctypes.byref(n_used))
+        self._check(rc, 'bb_bgzf_compress')
+        return self._bgzf_buf[:n_out.value], int(n_used.value)
 
     # ---- the one collective: SUM of emitted bases over the GPUs (stop condition, simulate.py:63)
     def comm_init_rank(self, unique_id, rank, world):

@@ -467,11 +467,21 @@ def _write_fastq(stdout, buf):
         stdout.write(bytes(buf).decode('latin-1'))
 
 
+def _binary(stdout):
+    """The binary layer of a real file / pipe, or the stream itself when it takes bytes (tests)."""
+    raw = getattr(stdout, 'buffer', None)
+    if raw is None:
+        return stdout
+    stdout.flush()
+    return raw
+
+
 def run_batches(args, ref, frag_lengths, identities, error_model, qscore_model, seed, target_size, n_gpus, output, stdout):
     """The driver loop of simulate.py:63-86 over batches of reads.  Reads are numbered 0, 1, 2, ...; a batch of B
     indices is dealt out over the GPUs (GPU g takes indices = g mod G), planned by the native planner, sequenced on
     the GPUs side by side (one host thread each) and written in index order until the total reaches the target, so
-    the FASTQ is independent of the batch size and of the number of GPUs."""
+    the FASTQ is independent of the batch size and of the number of GPUs.  With --gzip the GPUs compress the FASTQ to
+    BGZF (badread_b200/bgzf.py) before it is written."""
     from .planner import NativePlanner, fastq_format_sharded
     from ._lib import ReadResult
     import os
@@ -499,6 +509,10 @@ def run_batches(args, ref, frag_lengths, identities, error_model, qscore_model, 
     t_first = time.perf_counter()   # engines, reference and tables are resident: the simulate loop proper starts here
     out_buf = None
     empty = np.zeros(1, dtype=np.uint8)
+    writer = None
+    if getattr(args, 'gzip', False):
+        from .bgzf import BGZFWriter
+        writer = BGZFWriter(engines, _binary(stdout))
     print_progress(count, total_size, target_size, output)
     try:
         while total_size < target_size:
@@ -530,7 +544,10 @@ def run_batches(args, ref, frag_lengths, identities, error_model, qscore_model, 
             quals = [r.qual if r is not None else empty for r in results]
             buf, n_emit, bases, _, out_buf = fastq_format_sharded(planned, recs, seqs, quals, 0, total_size, target_size,
                                                                   out=out_buf)
-            _write_fastq(stdout, buf)
+            if writer is None:
+                _write_fastq(stdout, buf)
+            else:
+                writer.write(buf)
             if use_nccl:
                 # every GPU learns the batch's total from one all-reduce: more than was written means the target was
                 # reached inside this batch (the FASTQ stops after the read that reaches it, simulate.py:63)
@@ -540,6 +557,8 @@ def run_batches(args, ref, frag_lengths, identities, error_model, qscore_model, 
             count += n_emit
             print_progress(count, total_size, target_size, output)
             next_index += n_batch
+        if writer is not None:
+            writer.close()
         return {'reads': count, 'bases': total_size, 'gpus': n_gpus, 'batches_s': time.perf_counter() - t_first,
                 'nccl_stop_condition': bool(use_nccl)}
     finally:

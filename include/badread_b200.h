@@ -202,6 +202,23 @@ BB_API int bb_get_qscores(bb_ctx *ctx, uint64_t read_index, const uint8_t *seq, 
 BB_API int bb_align_path(bb_ctx *ctx, const uint8_t *query, int32_t q_len, const uint8_t *target, int32_t t_len,
                   uint8_t *ops_out, int64_t ops_cap, int64_t *n_ops, int32_t *distance);
 
+/* ---- BGZF output ------------------------------------------------------------------------------------ */
+/* FASTQ text compressed on the device as BGZF (SAM specification §4.1): independent gzip members of BB_BGZF_CHUNK input
+ * bytes each (the last one of a stream may be shorter), at fixed offsets of the whole stream, so the bytes do not depend on
+ * how the caller splits the stream into calls.  gzip, zlib and htslib read the result.  Each member is entropy coded with
+ * its own dynamic Huffman tables per sequence / quality segment (no string matching), or stored if that is not smaller.
+ *  bb_bgzf_bound(n): the most bytes compressing n input bytes can give (the end-of-file member not counted).
+ *  bb_bgzf_compress: line_mod4 is the index mod 4 of the FASTQ line in[0] belongs to.  Without `final` only the whole
+ *  chunks of in[0..n) are compressed and *n_consumed = their length: the caller keeps the rest and passes it again,
+ *  followed by more input, in the next call.  With `final` the last partial chunk is compressed as well (*n_consumed = n).
+ *  The 28-byte end-of-file member is never written: the caller appends it once the stream is complete.  out_cap must be at
+ *  least bb_bgzf_bound(bytes to be consumed), else BB_ERR_CAPACITY with *n_out = that bound.  *n_out = bytes written.
+ *  The call runs on a stream and scratch of the context's own: the batch workers' streams and buffers are left alone. */
+#define BB_BGZF_CHUNK 65280
+BB_API int64_t bb_bgzf_bound(int64_t n);
+BB_API int bb_bgzf_compress(bb_ctx *ctx, const uint8_t *in, int64_t n, int line_mod4, int final, uint8_t *out, int64_t out_cap,
+                            int64_t *n_out, int64_t *n_consumed);
+
 /* ---- host-side helpers (no GPU needed) -------------------------------------------------------------- */
 /* error_model.align_kmers (error_model.py:179-229) for a batch of (kmer, alt) pairs: kmers is n_alts*k bytes,
  * alts are concatenated with alt_off[n_alts+1]. Writes n_alts*k encoded slots, appends long strings to pool
