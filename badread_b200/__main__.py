@@ -1,7 +1,8 @@
 """
 Command line of badread_b200: `python -m badread_b200 simulate ...` with the flags, defaults and validation
 messages of `badread simulate` (/root/reference/badread/__main__.py:83-147, 239-336). Additive flags: --gpus,
---batch_reads. The model-building and plotting subcommands of Badread are outside this package's scope.
+--batch_reads. `error_model` and `qscore_model` take the reference's arguments, and their --alignment may also be SAM or
+BAM (then --reads is optional). The plotting subcommand of Badread is outside this package's scope.
 
 Derived from Badread (Copyright 2018 Ryan Wick, rrwick@gmail.com, https://github.com/rrwick/Badread), which is free
 software under the GNU General Public License version 3 or later; this file mirrors the named parts of the
@@ -44,16 +45,26 @@ def parse_args(args):
     if len(args) == 0:
         parser.print_help(file=sys.stderr)
         sys.exit(1)
-    return parser.parse_args(args)
+    parsed = parser.parse_args(args)
+    if parsed.subparser_name in ('error_model', 'qscore_model') and parsed.reads is None:
+        from .model_builders import alignment_format
+        if alignment_format(parsed.alignment) == 'paf':   # (SAM and BAM records can carry the reads)
+            subparsers.choices[parsed.subparser_name].error('the following arguments are required: --reads')
+    return parsed
 
 
 def model_subparser(subparsers, name, description, default_k):
-    """The arguments of `badread error_model` / `badread qscore_model` (__main__.py:150-208 of the reference)."""
+    """The arguments of `badread error_model` / `badread qscore_model` (__main__.py:150-208 of the reference); --alignment
+    may also be SAM or BAM, and then --reads may be left out."""
     group = subparsers.add_parser(name, description=description)
     required = group.add_argument_group('Required arguments')
     required.add_argument('--reference', type=str, required=True, help='Reference FASTA file')
-    required.add_argument('--reads', type=str, required=True, help='FASTQ of real reads')
-    required.add_argument('--alignment', type=str, required=True, help='PAF alignment of reads aligned to reference')
+    required.add_argument('--reads', type=str,
+                          help='FASTQ of real reads (optional for a SAM or BAM alignment: the reads are then taken from '
+                               'its records)')
+    required.add_argument('--alignment', type=str, required=True,
+                          help='Alignment of reads to the reference: PAF with cg:Z: and AS:i: tags, or SAM / BAM with '
+                               'AS:i: tags (told apart by content)')
     optional = group.add_argument_group('Optional arguments')
     what = 'error' if name == 'error_model' else 'qscore'
     optional.add_argument('--k_size', type=int, default=default_k,

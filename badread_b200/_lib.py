@@ -65,6 +65,14 @@ class PlanView(ctypes.Structure):
                 ('info', ctypes.c_void_p), ('frag_len', ctypes.c_void_p)]
 
 
+class AlnView(ctypes.Structure):
+    """bb_aln_view (include/badread_b200.h)."""
+    _fields_ = [('n_records', ctypes.c_int64), ('n_refs', ctypes.c_int32), ('n_reads', ctypes.c_int32)] + \
+        [(f, ctypes.c_void_p) for f in ('ref_names', 'ref_name_off', 'read_names', 'read_name_off', 'read_id', 'ref_id', 'flag',
+                                        'score', 'nm', 'read_len', 'read_start', 'read_end', 'columns', 'ref_start', 'ref_end',
+                                        'cigar', 'cigar_off', 'seq', 'qual', 'seq_off', 'has_qual', 'full')]
+
+
 class LibraryMissing(RuntimeError):
     pass
 
@@ -133,6 +141,10 @@ def lib():
         'bb_model_error': (c.c_char_p, []),
         'bb_bgzf_bound': (i64, [i64]),
         'bb_bgzf_compress': (c.c_int, [vp, vp, i64, c.c_int, c.c_int, vp, i64, P(i64), P(i64)]),
+        'bb_bgzf_decompress': (c.c_int, [c.c_int, vp, i64, vp, i64, P(i64)]),
+        'bb_aln_parse': (c.c_int, [vp, i64, c.c_int, i64, P(vp)]),
+        'bb_aln_view_get': (c.c_int, [vp, P(AlnView)]),
+        'bb_aln_free': (c.c_int, [vp]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(L, name)
@@ -151,4 +163,4 @@ EXPORTED_SYMBOLS = ['bb_create', 'bb_destroy', 'bb_last_error', 'bb_version', 'b
                     'bb_comm_init_all', 'bb_allreduce_bases', 'bb_allreduce_bases_all', 'bb_planner_create', 'bb_planner_destroy',
                     'bb_planner_plan', 'bb_planner_view', 'bb_planner_error', 'bb_fastq_format', 'bb_fastq_format_sharded',
                     'bb_count_kmer_alternatives', 'bb_count_kmer_alternatives_wide', 'bb_count_cigar_qscores', 'bb_model_error',
-                    'bb_bgzf_bound', 'bb_bgzf_compress']
+                    'bb_bgzf_bound', 'bb_bgzf_compress', 'bb_bgzf_decompress', 'bb_aln_parse', 'bb_aln_view_get', 'bb_aln_free']

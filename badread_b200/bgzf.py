@@ -1,18 +1,43 @@
 """
-BGZF output of `simulate --gzip`: FASTQ records compressed on the GPUs (Engine.bgzf_compress, csrc/bb_bgzf.cuh) and
-written as BGZF (SAM specification §4.1), which gzip, zlib and htslib read.
+BGZF (SAM specification §4.1) on the GPU, both ways.
 
-Members hold BGZF_CHUNK bytes at fixed offsets of the whole FASTQ stream: the writer carries the tail of every buffer
-into the next one, so the compressed bytes depend neither on the batch size nor on the number of GPUs.
+Output of `simulate --gzip`: FASTQ records compressed on the GPUs (Engine.bgzf_compress, csrc/bb_bgzf.cuh) and written as
+BGZF, which gzip, zlib and htslib read.  Members hold BGZF_CHUNK bytes at fixed offsets of the whole FASTQ stream: the
+writer carries the tail of every buffer into the next one, so the compressed bytes depend neither on the batch size nor
+on the number of GPUs.
+
+Input (`decompress`): a whole BGZF file, BAM for the model builders, inflated on one GPU, one warp per member
+(csrc/bb_inflate.cuh).
 """
+import ctypes
 import threading
 
 import numpy as np
 
+from . import _lib
 from ._lib import BB_BGZF_CHUNK as BGZF_CHUNK
 
 # the empty member that ends a BGZF file (SAM specification §4.1.2)
 EOF_MEMBER = bytes.fromhex('1f8b08040000000000ff0600424302001b0003000000000000000000')
+
+
+def decompress(data, device=0):
+    """The inflated bytes (a bytearray) of the BGZF stream `data` (bytes-like), inflated on GPU `device`.  Raises ValueError
+    with the library's message for input that is not BGZF or a member that is corrupt (named by index and offset)."""
+    L = _lib.lib()
+    src = np.frombuffer(memoryview(data).cast('B'), dtype=np.uint8)
+    src_ptr = src.ctypes.data_as(ctypes.c_void_p) if src.size else None
+    n_out = ctypes.c_int64(0)
+    rc = L.bb_bgzf_decompress(device, src_ptr, src.size, None, 0, ctypes.byref(n_out))
+    out = bytearray(n_out.value)
+    if rc == _lib.BB_ERR_CAPACITY:
+        rc = L.bb_bgzf_decompress(device, src_ptr, src.size, (ctypes.c_char * len(out)).from_buffer(out), len(out),
+                                  ctypes.byref(n_out))
+    if rc == _lib.BB_ERR_ARG:
+        raise ValueError(L.bb_model_error().decode(errors='replace'))
+    if rc != _lib.BB_OK:
+        raise RuntimeError('bgzf.decompress: ' + L.bb_model_error().decode(errors='replace'))
+    return out
 
 
 def _newlines(buf):

@@ -18,6 +18,8 @@
 #endif
 #include <cstdint>
 
+#include "bb_crc32.cuh"
+
 #define BGZF_CHUNK 65280           // input bytes per member (htslib's BGZF_BLOCK_SIZE)
 #define BGZF_SLOT 65536            // bytes of a member's slot in the scratch, and the largest member BGZF allows
 #define BGZF_THREADS 256
@@ -53,30 +55,8 @@ struct BGZFSmem {
 };
 #define BGZF_SMEM_BYTES ((int)sizeof(BGZFSmem))
 
-#define BGZF_POLY 0xedb88320u
-
 // order in which a dynamic block header lists the code lengths of the code-length code
 __constant__ uint8_t bgzf_c_cl_order[BGZF_NCL] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
-
-// a * b modulo the CRC-32 polynomial, both reflected (bit 31 is x^0)
-__device__ __forceinline__ uint32_t bgzf_mulmod(uint32_t a, uint32_t b) {
-    uint32_t p = 0;
-    for (int i = 0; i < 32; i++) {
-        if (a & (0x80000000u >> i)) p ^= b;
-        b = (b >> 1) ^ ((b & 1u) ? BGZF_POLY : 0u);
-    }
-    return p;
-}
-
-// x^(8 n) modulo the polynomial: appending n zero bytes to a message multiplies its CRC register by this
-__device__ __forceinline__ uint32_t bgzf_x8n(uint32_t n) {
-    uint32_t r = 0x80000000u, sq = 1u << 23;   // x^0, x^8
-    for (; n; n >>= 1) {
-        if (n & 1u) r = bgzf_mulmod(r, sq);
-        sq = bgzf_mulmod(sq, sq);
-    }
-    return r;
-}
 
 // Exclusive prefix sum over the CTA; *total = the sum of all threads' values.  Every thread must call it.
 __device__ __forceinline__ uint32_t bgzf_scan(BGZFSmem &s, uint32_t v, uint32_t *total) {
@@ -292,9 +272,7 @@ bgzf_k_compress(const uint8_t *__restrict__ in, int64_t n, const int64_t *__rest
         for (int i = t; i < n16; i += BGZF_THREADS) reinterpret_cast<uint4 *>(s.in)[i] = reinterpret_cast<const uint4 *>(src)[i];
         for (int i = (n16 << 4) + t; i < len; i += BGZF_THREADS) s.in[i] = src[i];
         for (int i = t; i < BGZF_SLOT / 4; i += BGZF_THREADS) s.out[i] = 0;
-        uint32_t e = (uint32_t)t;
-        for (int k = 0; k < 8; k++) e = (e >> 1) ^ ((e & 1u) ? BGZF_POLY : 0u);
-        s.crc_table[t] = e;
+        s.crc_table[t] = bgzf_crc_entry((uint32_t)t);
     }
     __syncthreads();
 

@@ -1,0 +1,76 @@
+// bb_tu_inflate.cu — compiles the BGZF inflater (bb_inflate.cuh) and its C ABI entry point, bb_bgzf_decompress.
+// Like the model builders' calls it takes a device instead of a context and reports errors through bb_model_error().
+#include <cuda_runtime.h>
+
+#include <cstdint>
+#include <cstdio>
+#include <vector>
+
+#include "../../include/badread_b200.h"
+
+#include "bb_inflate.cuh"
+
+void bbm_set_error(const char *msg);   // bb_tu_models.cu
+
+namespace {
+
+struct DevBuf {   // released on every exit path
+    void *p = nullptr;
+    ~DevBuf() { if (p) cudaFree(p); }
+};
+
+int cuda_fail(const char *what, cudaError_t e) {
+    char msg[256];
+    std::snprintf(msg, sizeof(msg), "bb_bgzf_decompress: %s: %s", what, cudaGetErrorString(e));
+    bbm_set_error(msg);
+    return BB_ERR_CUDA;
+}
+
+}  // namespace
+
+#define BBI_TRY(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return cuda_fail(#call, e_); } while (0)
+
+extern "C" int bb_bgzf_decompress(int device, const uint8_t *in, int64_t n, uint8_t *out, int64_t out_cap, int64_t *n_out) {
+    bbm_set_error("");
+    char msg[256];
+    if (n < 0 || (n > 0 && !in) || !n_out || out_cap < 0 || (out_cap > 0 && !out)) {
+        bbm_set_error("bb_bgzf_decompress: invalid argument");
+        return BB_ERR_ARG;
+    }
+    std::vector<InflMember> members;
+    int64_t total = 0;
+    if (!infl_walk(in, n, members, &total, msg, sizeof(msg))) {
+        bbm_set_error(msg);
+        return BB_ERR_ARG;
+    }
+    *n_out = total;
+    if (total > out_cap) {
+        std::snprintf(msg, sizeof(msg), "bb_bgzf_decompress: %lld bytes of output, capacity %lld", (long long)total,
+                      (long long)out_cap);
+        bbm_set_error(msg);
+        return BB_ERR_CAPACITY;
+    }
+    if (members.empty()) return BB_OK;
+    const int64_t n_members = (int64_t)members.size();
+    BBI_TRY(cudaSetDevice(device));
+    (void)cudaGetLastError();   // (report this call's launch only)
+    DevBuf d_in, d_out, d_members, d_status;
+    BBI_TRY(cudaMalloc(&d_in.p, (size_t)n));
+    BBI_TRY(cudaMalloc(&d_out.p, (size_t)(total ? total : 16)));
+    BBI_TRY(cudaMalloc(&d_members.p, members.size() * sizeof(InflMember)));
+    BBI_TRY(cudaMalloc(&d_status.p, members.size() * sizeof(int32_t)));
+    BBI_TRY(cudaMemcpy(d_in.p, in, (size_t)n, cudaMemcpyHostToDevice));
+    BBI_TRY(cudaMemcpy(d_members.p, members.data(), members.size() * sizeof(InflMember), cudaMemcpyHostToDevice));
+    const int64_t grid = (n_members + INFL_WARPS - 1) / INFL_WARPS;
+    infl_k_members<<<(unsigned)grid, INFL_THREADS>>>((const uint8_t *)d_in.p, (const InflMember *)d_members.p, n_members,
+                                                      (uint8_t *)d_out.p, (int32_t *)d_status.p);
+    BBI_TRY(cudaGetLastError());
+    std::vector<int32_t> status(members.size());
+    BBI_TRY(cudaMemcpy(status.data(), d_status.p, members.size() * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    if (infl_first_failure(members, status.data(), msg, sizeof(msg))) {
+        bbm_set_error(msg);
+        return BB_ERR_ARG;
+    }
+    BBI_TRY(cudaMemcpy(out, d_out.p, (size_t)total, cudaMemcpyDeviceToHost));
+    return BB_OK;
+}

@@ -148,6 +148,9 @@ int count_common(bool qscores, bool wide, int device, int k, int max_del, int32_
 
 }  // namespace
 
+// the message of bb_model_error() for the calling thread, set by the other model-builder inputs (BGZF, SAM / BAM)
+void bbm_set_error(const char *msg) { std::snprintf(g_model_error, sizeof(g_model_error), "%s", msg); }
+
 extern "C" const char *bb_model_error(void) { return g_model_error; }
 
 extern "C" int bb_count_kmer_alternatives(int device, int k, int32_t n_aln, const uint8_t *read, const int64_t *read_off,

@@ -8,15 +8,21 @@ The host parses the three input files and flattens the chosen alignments; libbad
 (csrc/bb_tu_models.cu: one CTA per alignment, one thread per window, 64-bit keys in an open-addressing table with the
 first occurrence of every key); the host sorts and prints.  Windows whose content does not fit a key come back in an
 overflow list and are evaluated here, exactly, from the same flat arrays.
+
+The alignments may also be SAM (plain or gzipped) or BAM, told apart from PAF by their content (alignment_format).  A
+BAM's BGZF members are inflated on the GPU (bgzf.decompress); native host code (csrc/bb_bam.cpp) turns the records of
+either into the fields of the PAF line the reference would read, and the best alignment per read is chosen here with
+the rules of load_alignments, over arrays.  Without --reads the sequences and qualities come from the records.
 """
 import collections
 import ctypes
+import gzip
 import re
 import sys
 
 import numpy as np
 
-from . import _lib
+from . import _lib, bgzf
 from .misc import float_to_str, get_open_func, load_fasta, reverse_complement
 
 _CIGAR_RUN = re.compile(r'(\d+)([A-Za-z=])')
@@ -110,6 +116,177 @@ def load_alignments(filename, max_alignments=None, output=sys.stderr, dot_interv
                 print('.', end='', file=output, flush=True)
     print('', file=output, flush=True)
     return chosen
+
+
+_SAM_CIGAR = re.compile(r'(\d+[MIDNSHP=X])+')
+_inflate = bgzf.decompress      # BAM's BGZF, inflated on the GPU
+
+
+def alignment_format(filename):
+    """'bam', 'sam' or 'paf', from the content: BGZF whose first inflated bytes are BAM's magic is BAM; a first line that
+    starts with '@', or that has SAM's 11 columns with integer FLAG, POS and MAPQ and a CIGAR or '*' in column 6, is SAM
+    (plain or gzipped); anything else is PAF."""
+    try:
+        with open(filename, 'rb') as f:
+            magic = f.read(4)
+        with (gzip.open if magic[:2] == b'\x1f\x8b' else open)(filename, 'rb') as f:
+            head = f.read(4)
+            line = head + (f.readline() if not head.endswith(b'\n') else b'')
+    except (OSError, EOFError):
+        return 'paf'    # (unreadable: the PAF path reports it as it always has)
+    if magic == b'\x1f\x8b\x08\x04' and head == b'BAM\x01':
+        return 'bam'
+    if line.startswith(b'@'):
+        return 'sam'
+    f = line.rstrip(b'\r\n').split(b'\t')
+    if len(f) >= 11 and all(re.fullmatch(rb'-?\d+', f[i]) for i in (1, 3, 4)) and \
+            (f[5] == b'*' or _SAM_CIGAR.fullmatch(f[5].decode('latin-1'))):
+        return 'sam'
+    return 'paf'
+
+
+class SamAlignment(object):
+    """The chosen alignment of a read from a SAM / BAM record: the attributes of Alignment that FlatAlignments reads."""
+    __slots__ = ('read_name', 'read_start', 'read_end', 'strand', 'ref_name', 'ref_start', 'ref_end', 'runs')
+
+    def __init__(self, read_name, read_start, read_end, strand, ref_name, ref_start, ref_end, runs):
+        self.read_name, self.read_start, self.read_end, self.strand = read_name, read_start, read_end, strand
+        self.ref_name, self.ref_start, self.ref_end, self.runs = ref_name, ref_start, ref_end, runs
+
+
+def _view_array(ptr, n, dtype):
+    if n == 0:
+        return np.zeros(0, dtype=dtype)
+    return np.ctypeslib.as_array(ctypes.cast(ptr, ctypes.POINTER(np.ctypeslib.as_ctypes_type(dtype))), shape=(n,)).copy()
+
+
+def _names(blob_ptr, off):
+    blob = ctypes.string_at(blob_ptr, int(off[-1])) if off[-1] else b''
+    return [blob[a:b].decode() for a, b in zip(off[:-1].tolist(), off[1:].tolist())]
+
+
+def load_sam_alignments(filename, fmt, max_alignments, reads, refs, need_qual, output=sys.stderr, dot_interval=1000):
+    """The alignments of a SAM or BAM file, chosen as load_alignments chooses them: per read the record with the highest
+    AS:i (the last among equals), kept with more than 100 columns and more than 80 % identity, reads in order of first
+    appearance; --max_alignments counts mapped records.  The identity is (columns - NM:i) / columns, the matching bases
+    counted from the sequences only for a record without NM.  reads: the FASTQ's {name: (seq, qual)}, or None to take
+    every chosen read's sequence and qualities from a record of it that holds the whole read (SEQ not '*', no H clip),
+    turned back to the read's own orientation.  Returns (alignments, reads)."""
+    print('Loading alignments', end='', file=output, flush=True)
+    with (open if fmt == 'bam' else get_open_func(filename))(filename, 'rb') as handle:
+        data = handle.read()
+    if fmt == 'bam':
+        try:
+            data = _inflate(data)
+        except ValueError as e:
+            sys.exit(f'\nError: {filename} is not a valid BAM file ({e})')
+    L = _lib.lib()
+    buf = np.frombuffer(memoryview(data).cast('B'), dtype=np.uint8)
+    handle = ctypes.c_void_p()
+    rc = L.bb_aln_parse(buf.ctypes.data_as(ctypes.c_void_p) if buf.size else None, buf.size, int(fmt == 'bam'),
+                        max_alignments or 0, ctypes.byref(handle))
+    if rc != _lib.BB_OK:
+        sys.exit('\n' + L.bb_model_error().decode(errors='replace'))
+    try:
+        v = _lib.AlnView()
+        L.bb_aln_view_get(handle, ctypes.byref(v))
+        n = v.n_records
+        ref_names = _names(v.ref_names, _view_array(v.ref_name_off, v.n_refs + 1, np.int64))
+        read_names = _names(v.read_names, _view_array(v.read_name_off, v.n_reads + 1, np.int64))
+        a = {f: _view_array(getattr(v, f), n, t) for f, t in
+             (('read_id', np.int32), ('ref_id', np.int32), ('flag', np.int32), ('score', np.int32), ('nm', np.int32),
+              ('read_start', np.int32), ('read_end', np.int32), ('columns', np.int32), ('ref_start', np.int64),
+              ('ref_end', np.int64), ('has_qual', np.uint8), ('full', np.uint8))}
+        cigar_off = _view_array(v.cigar_off, n + 1, np.int64)
+        cigar = _view_array(v.cigar, int(cigar_off[-1]), np.uint32)
+        seq_off = _view_array(v.seq_off, n + 1, np.int64)
+        seq = ctypes.string_at(v.seq, int(seq_off[-1])) if seq_off[-1] else b''
+        qual = ctypes.string_at(v.qual, int(seq_off[-1])) if seq_off[-1] else b''
+    finally:
+        L.bb_aln_free(handle)
+    print('.' * (n // dot_interval), file=output, flush=True)
+
+    print('Choosing best alignment per read', end='', file=output, flush=True)
+    order = np.lexsort((np.arange(n), a['score'], a['read_id']))           # per read: by score, then by position
+    last = np.flatnonzero(np.append(a['read_id'][order][1:] != a['read_id'][order][:-1], True)) if n else order
+    best = order[last]                                                      # reads in order of first appearance
+
+    def whole_read(i):
+        """The read of record i's own orientation from the record of it that holds the whole read."""
+        rid = int(a['read_id'][i])
+        name = read_names[rid]
+        if reads is not None:
+            return reads.get(name)
+        j = full_of.get(rid)
+        if j is None:
+            sys.exit(f'\nError: no record of read {name} holds its whole sequence (SEQ not * and no hard clips): '
+                     f'give the reads with --reads')
+        if need_qual and not a['has_qual'][j]:
+            sys.exit(f'\nError: the record of read {name} has no qualities (QUAL is *): give the reads with --reads')
+        s = seq[seq_off[j]:seq_off[j + 1]].decode('latin-1')
+        q = qual[seq_off[j]:seq_off[j + 1]].decode('latin-1') if a['has_qual'][j] else ''
+        if a['flag'][j] & 16:
+            s, q = reverse_complement(s), q[::-1]
+        return s, q
+
+    full_idx = np.flatnonzero(a['full'])
+    _, first_full = np.unique(a['read_id'][full_idx], return_index=True)
+    full_of = dict(zip(a['read_id'][full_idx][first_full].tolist(), full_idx[first_full].tolist()))
+    matches = a['columns'][best].astype(np.int64) - a['nm'][best]
+    own_reads = {} if reads is None else reads
+    for k in np.flatnonzero(a['nm'][best] < 0).tolist():                    # no NM:i: count from the sequences
+        i = int(best[k])
+        matches[k] = _count_matches(i, a, cigar, cigar_off, whole_read(i), refs.get(ref_names[a['ref_id'][i]]))
+    cols = a['columns'][best].astype(np.int64)
+    with np.errstate(divide='ignore', invalid='ignore'):
+        keep = best[(cols > 100) & (100.0 * matches / cols > 80.0)]
+    chosen = []
+    for i in keep.tolist():
+        name = read_names[a['read_id'][i]]
+        if reads is None and name not in own_reads:
+            own_reads[name] = whole_read(i)
+        runs = [(c >> 4, 'MIDNSHPMM'[c & 15]) for c in cigar[cigar_off[i]:cigar_off[i + 1]].tolist() if (c & 15) not in (4, 5)]
+        strand = '-' if a['flag'][i] & 16 else '+'
+        if strand == '-':
+            runs.reverse()
+        chosen.append(SamAlignment(name, int(a['read_start'][i]), int(a['read_end'][i]), strand, ref_names[a['ref_id'][i]],
+                                   int(a['ref_start'][i]), int(a['ref_end'][i]), runs))
+        if len(chosen) % dot_interval == 0:
+            print('.', end='', file=output, flush=True)
+    print('', file=output, flush=True)
+    return chosen, own_reads
+
+
+def _count_matches(i, a, cigar, cigar_off, read, ref):
+    """Matching bases of record i without NM:i: its M = X columns where the read (in the reference's orientation) and the
+    reference agree."""
+    if read is None or ref is None:
+        return 0        # (FlatAlignments reports the missing read or reference)
+    seq = read[0]
+    s = reverse_complement(seq) if a['flag'][i] & 16 else seq
+    rp, fp, m = 0, int(a['ref_start'][i]), 0
+    for c in cigar[cigar_off[i]:cigar_off[i + 1]].tolist():
+        op, n = c & 15, c >> 4
+        if op in (0, 7, 8):
+            m += sum(x == y for x, y in zip(s[rp:rp + n], ref[fp:fp + n]))
+            rp += n
+            fp += n
+        elif op in (1, 4, 5):     # (the whole read holds the hard-clipped bases too)
+            rp += n
+        elif op == 2:
+            fp += n
+    return m
+
+
+def load_inputs(args, refs, output, need_qual):
+    """(reads, chosen alignments) of the builders' --reads and --alignment, whichever alignment format it is (--reads may
+    be None for SAM and BAM only)."""
+    fmt = alignment_format(args.alignment)
+    reads = load_fastq(args.reads, output=output) if args.reads is not None else None
+    if fmt == 'paf':
+        return reads, load_alignments(args.alignment, args.max_alignments, output=output)
+    alignments, reads = load_sam_alignments(args.alignment, fmt, args.max_alignments, reads, refs, need_qual, output=output)
+    return reads, alignments
 
 
 class FlatAlignments(object):
@@ -311,8 +488,7 @@ def _error_model_lines_sparse(args, flat, k):
 def make_error_model(args, output=sys.stderr, dot_interval=1000):
     """error_model.py:31-83."""
     refs = load_fasta(args.reference)[0]
-    reads = load_fastq(args.reads, output=output)
-    alignments = load_alignments(args.alignment, args.max_alignments, output=output)
+    reads, alignments = load_inputs(args, refs, output, need_qual=False)
     if len(alignments) == 0:
         sys.exit('Error: no usable alignments')
     k = args.k_size
@@ -384,8 +560,7 @@ def print_qscore_fractions(cigar, qscores, min_occur):
 def make_qscore_model(args, output=sys.stderr, dot_interval=1000):
     """qscore_model.py:78-161."""
     refs = load_fasta(args.reference)[0]
-    reads = load_fastq(args.reads, output=output)
-    alignments = load_alignments(args.alignment, args.max_alignments, output=output)
+    reads, alignments = load_inputs(args, refs, output, need_qual=True)
     if len(alignments) == 0:
         sys.exit('Error: no usable alignments')
     assert args.k_size % 2 == 1     # an odd size has a middle base to take the qscore from

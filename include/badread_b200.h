@@ -219,6 +219,17 @@ BB_API int64_t bb_bgzf_bound(int64_t n);
 BB_API int bb_bgzf_compress(bb_ctx *ctx, const uint8_t *in, int64_t n, int line_mod4, int final, uint8_t *out, int64_t out_cap,
                             int64_t *n_out, int64_t *n_consumed);
 
+/* ---- BGZF input ------------------------------------------------------------------------------------- */
+/* Inflates the BGZF stream in[0..n) on `device` (any number of members, the end-of-file member included) into out: one warp
+ * per member, all three deflate block types, every member's CRC-32 and ISIZE checked.  Like the model builders' calls it
+ * takes a device instead of a bb_ctx, allocates and releases what it needs, and describes failures in bb_model_error().
+ *  The host walks the members' BC extra fields (BSIZE) first: *n_out = the inflated size of the stream (the sum of the
+ *  ISIZEs); BB_ERR_CAPACITY if out_cap is smaller (out may then be NULL).
+ *  BB_ERR_ARG for input that is not BGZF (a gzip member without BC) and for a member that is truncated, holds an invalid
+ *  Huffman table or code, a back-reference before its start, or does not match its CRC-32 or ISIZE; the message names the
+ *  member (index and offset).  Malformed input never makes the kernel read or write outside the member. */
+BB_API int bb_bgzf_decompress(int device, const uint8_t *in, int64_t n, uint8_t *out, int64_t out_cap, int64_t *n_out);
+
 /* ---- host-side helpers (no GPU needed) -------------------------------------------------------------- */
 /* error_model.align_kmers (error_model.py:179-229) for a batch of (kmer, alt) pairs: kmers is n_alts*k bytes,
  * alts are concatenated with alt_off[n_alts+1]. Writes n_alts*k encoded slots, appends long strings to pool
@@ -354,6 +365,33 @@ BB_API int bb_count_cigar_qscores(int device, int k, int max_del, int32_t n_aln,
                            uint64_t *overall_out, int64_t ovf_cap, int32_t *ovf_aln, int32_t *ovf_pos, int32_t *ovf_k,
                            int64_t *n_ovf);
 BB_API const char *bb_model_error(void);
+
+/* SAM / BAM alignment records for the model builders, parsed on the host (no GPU needed).  data[0..n) is SAM text or, with
+ * is_bam, an inflated BAM file (bb_bgzf_decompress).  Mapped records only (FLAG 0x4 and RNAME '*' / refID -1 are skipped),
+ * at most max_records of them (<= 0: all).  Per record the fields of the PAF line the reference's builders read:
+ *   read_len    the M I S = X H ops            read_start  the leading clip (S + H) on '+', the trailing clip on '-'
+ *   read_end    read_start + the M I = X ops   ref_start   POS - 1;   ref_end  ref_start + the M D = X ops
+ *   columns     the M I D = X ops              nm          NM:i, or -1 without it;   score  AS:i
+ * and the CIGAR runs (length << 4 | BAM op code, SAM order), SEQ (upper case) and QUAL (Phred+33) as stored; a record
+ * without SEQ has none, has_qual[i] = 0 without QUAL, full[i] = SEQ present and no H clip.  Reads and references are
+ * numbered in order of first appearance (references of a BAM header or of SAM @SQ lines first).
+ * BB_ERR_ARG with bb_model_error() = the message to exit with: "Error: no CIGAR string found" (a mapped record with
+ * CIGAR '*'), "Error: no alignment score" (no AS:i), an N or P op (names the read), or malformed input. */
+typedef struct bb_aln_set bb_aln_set;
+typedef struct bb_aln_view {
+    int64_t n_records;
+    int32_t n_refs, n_reads;
+    const char *ref_names;  const int64_t *ref_name_off;    /* [n_refs + 1] */
+    const char *read_names; const int64_t *read_name_off;   /* [n_reads + 1] */
+    const int32_t *read_id, *ref_id, *flag, *score, *nm, *read_len, *read_start, *read_end, *columns;   /* [n_records] */
+    const int64_t *ref_start, *ref_end;                     /* [n_records] */
+    const uint32_t *cigar;  const int64_t *cigar_off;       /* [n_records + 1] */
+    const uint8_t *seq, *qual; const int64_t *seq_off;      /* [n_records + 1] */
+    const uint8_t *has_qual, *full;                         /* [n_records] */
+} bb_aln_view;
+BB_API int bb_aln_parse(const uint8_t *data, int64_t n, int is_bam, int64_t max_records, bb_aln_set **set);
+BB_API int bb_aln_view_get(const bb_aln_set *set, bb_aln_view *view);   /* valid until bb_aln_free */
+BB_API int bb_aln_free(bb_aln_set *set);
 
 #ifdef __cplusplus
 }
