@@ -370,17 +370,19 @@ def _ptr(a):
     return a.ctypes.data_as(ctypes.c_void_p)
 
 
-def _count(which, flat, k, max_del=0, device=0):
+def _count(which, flat, k, max_del=0, device=0, cap=None, ovf_cap=None):
     """Runs bb_count_kmer_alternatives ('kmers'), bb_count_kmer_alternatives_wide ('kmers_wide': keys come back as
     (n, 2) words, read k-mer and reference k-mer << 6 | length) or bb_count_cigar_qscores ('cigars'), growing the table
-    until it fits."""
+    (from `cap` slots, a power of two >= 16) and the overflow list (from `ovf_cap` entries) until they fit."""
     L = _lib.lib()
     per_slot = N_Q if which == 'cigars' else 1
     key_words = 2 if which == 'kmers_wide' else 1
-    cap = 1 << 18       # slots; doubled until the distinct keys fit (k-mer pairs: at most one per window)
-    while which != 'cigars' and cap < min(2 * int(flat.ref_off[-1]) + 16, 1 << 22):
-        cap <<= 1
-    ovf_cap = 1 << 16
+    if cap is None:
+        cap = 1 << 18       # slots; doubled until the distinct keys fit (k-mer pairs: at most one per window)
+        while which != 'cigars' and cap < min(2 * int(flat.ref_off[-1]) + 16, 1 << 22):
+            cap <<= 1
+    if ovf_cap is None:
+        ovf_cap = 1 << 16
     while True:
         keys = np.empty(cap * key_words, dtype=np.uint64); first = np.empty(cap, dtype=np.uint64)
         counts = np.empty(cap * per_slot, dtype=np.uint32)
