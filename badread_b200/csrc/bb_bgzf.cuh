@@ -88,8 +88,9 @@ __device__ __forceinline__ void bgzf_put(uint32_t *out, uint32_t pos, uint32_t v
 
 // Huffman code lengths of at most max_len bits for the n symbols of freq[] (at least two of them non-zero): the
 // lengths of a Huffman tree, lengths beyond max_len cut and the overflow of the Kraft sum paid back by lengthening the
-// longest shorter codes, then handed out again so that a less frequent symbol (ties: the higher symbol) never gets a
-// shorter code.  Every thread calls it; one thread builds the tree.
+// longest shorter codes, then handed out again by rank, leaves ranked by (frequency, symbol) and the longest lengths
+// to the lowest ranks: a less frequent symbol never gets a shorter code, and of two equally frequent symbols the lower
+// one never gets the shorter code.  Every thread calls it; one thread builds the tree.
 __device__ void bgzf_code_lengths(BGZFSmem &s, const uint32_t *freq, int n, int max_len, uint8_t *lens) {
     for (int i = threadIdx.x; i < n; i += BGZF_THREADS) {
         const uint32_t f = freq[i];

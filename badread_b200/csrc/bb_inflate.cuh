@@ -27,7 +27,7 @@
 
 enum InflStatus {
     INFL_OK = 0, INFL_TRUNCATED = 1, INFL_BAD_BLOCK = 2, INFL_BAD_STORED = 3, INFL_BAD_TABLE = 4, INFL_BAD_CODE = 5,
-    INFL_BAD_DISTANCE = 6, INFL_OVERRUN = 7, INFL_SHORT = 8, INFL_BAD_CRC = 9
+    INFL_BAD_DISTANCE = 6, INFL_OVERRUN = 7, INFL_SHORT = 8, INFL_BAD_CRC = 9, INFL_TRAILING = 10
 };
 
 struct InflMember {      // one member, from the host walk
@@ -227,6 +227,8 @@ __device__ int infl_member(const uint8_t *in, int32_t n, uint8_t *out, int32_t i
             for (int i = 0; i < len; i++, pos++) out[pos] = out[pos - dist];
         }
     } while (!last);
+    // the trailer follows the final block's last byte: zlib and gzip refuse bytes in between (they read them as CRC-32)
+    if (((int64_t)b.pos * 8 - b.cnt + 7) / 8 < n) return INFL_TRAILING;
     return pos == isize ? INFL_OK : INFL_SHORT;
 }
 
@@ -272,6 +274,7 @@ inline const char *infl_status_text(int st) {
         case INFL_OVERRUN: return "more data than the ISIZE of the trailer";
         case INFL_SHORT: return "less data than the ISIZE of the trailer";
         case INFL_BAD_CRC: return "CRC-32 mismatch";
+        case INFL_TRAILING: return "bytes between the final deflate block and the trailer";
         default: return "ok";
     }
 }
