@@ -131,6 +131,8 @@ def simulate_subparser(subparsers):
                            help='Reads per GPU per batch (default: %(default)s)')
     b200_args.add_argument('--gzip', action='store_true',
                            help='Write the FASTQ as BGZF (gzip-compatible), compressed on the GPUs')
+    b200_args.add_argument('--bam', action='store_true',
+                           help='Write unaligned BAM instead of FASTQ, built and compressed on the GPUs')
     group.add_argument('--version', action='version', version='Badread v' + __version__)
 
 
@@ -204,6 +206,8 @@ def check_simulate_args(args):
         args.error_model = args.error_model.lower() if args.error_model.lower() == args.error_model else args.error_model
     if getattr(args, 'gpus', 1) < 1:
         sys.exit('Error: --gpus must be at least 1')
+    if getattr(args, 'bam', False) and getattr(args, 'gzip', False):
+        sys.exit('Error: --bam and --gzip cannot be used together (BAM is always compressed)')
 
 
 def check_beta_identities(args):

@@ -39,6 +39,12 @@ class ReadResult(ctypes.Structure):
                 ('loop_kcycles', ctypes.c_int32), ('align_kcycles', ctypes.c_int32)]
 
 
+class BamRecord(ctypes.Structure):
+    """bb_bam_record (include/badread_b200.h)."""
+    _fields_ = [('out_off', ctypes.c_int64), ('text_off', ctypes.c_int64), ('out_len', ctypes.c_int32),
+                ('name_len', ctypes.c_int32), ('co_len', ctypes.c_int32), ('reserved', ctypes.c_int32)]
+
+
 class PlanConfig(ctypes.Structure):
     """bb_plan_config (include/badread_b200.h)."""
     _fields_ = [('seed', ctypes.c_uint64), ('n_contigs', ctypes.c_int32), ('contig_len', ctypes.c_void_p),
@@ -142,6 +148,13 @@ def lib():
         'bb_bgzf_bound': (i64, [i64]),
         'bb_bgzf_compress': (c.c_int, [vp, vp, i64, c.c_int, c.c_int, vp, i64, P(i64), P(i64)]),
         'bb_bgzf_decompress': (c.c_int, [c.c_int, vp, i64, vp, i64, P(i64)]),
+        'bb_fetch_last_batch_results': (c.c_int, [vp, vp, P(i64)]),
+        'bb_bam_build': (c.c_int, [vp, i32, vp, vp, i64]),
+        'bb_bam_compress_device': (c.c_int, [vp, c.c_int, vp, i64, P(i64)]),
+        'bb_bam_fetch_records': (c.c_int, [vp, vp, vp, i64, P(i64)]),
+        'bb_bam_compress': (c.c_int, [vp, vp, i64, i64, vp, i64, c.c_int, vp, i64, P(i64), P(i64)]),
+        'bb_bam_layout_sharded': (c.c_int, [i32, vp, vp, i32, i64, i64, i64, vp, vp, vp, vp, vp, vp, i64, P(i64), P(i64),
+                                            P(i32), P(i64), P(i32)]),
         'bb_aln_parse': (c.c_int, [vp, i64, c.c_int, i64, P(vp)]),
         'bb_aln_view_get': (c.c_int, [vp, P(AlnView)]),
         'bb_aln_free': (c.c_int, [vp]),
@@ -163,4 +176,6 @@ EXPORTED_SYMBOLS = ['bb_create', 'bb_destroy', 'bb_last_error', 'bb_version', 'b
                     'bb_comm_init_all', 'bb_allreduce_bases', 'bb_allreduce_bases_all', 'bb_planner_create', 'bb_planner_destroy',
                     'bb_planner_plan', 'bb_planner_view', 'bb_planner_error', 'bb_fastq_format', 'bb_fastq_format_sharded',
                     'bb_count_kmer_alternatives', 'bb_count_kmer_alternatives_wide', 'bb_count_cigar_qscores', 'bb_model_error',
-                    'bb_bgzf_bound', 'bb_bgzf_compress', 'bb_bgzf_decompress', 'bb_aln_parse', 'bb_aln_view_get', 'bb_aln_free']
+                    'bb_bgzf_bound', 'bb_bgzf_compress', 'bb_bgzf_decompress', 'bb_aln_parse', 'bb_aln_view_get', 'bb_aln_free',
+                    'bb_fetch_last_batch_results', 'bb_bam_build', 'bb_bam_compress_device', 'bb_bam_fetch_records',
+                    'bb_bam_compress', 'bb_bam_layout_sharded']

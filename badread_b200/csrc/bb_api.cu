@@ -216,11 +216,29 @@ struct bb_ctx {
     int64_t *h_bgzf = nullptr;   // pinned: line_pref[n_chunks] and offsets[n_chunks] of the last pass
     DevBuf bgzf_in, bgzf_slots, bgzf_lines, bgzf_sizes, bgzf_pref, bgzf_off, bgzf_out;
 
+    // BAM output (bb_bam_*), on bgzf_stream.  The last fetched batch: its workers' blocks start at out_base[w] of the
+    // concatenated output (out_base[n_split] = its size).
+    bool fetched = false;
+    std::vector<int64_t> out_base;
+    // The record stream bytes [bam_base, bam_base + bam_len) in bam_buf[bam_cur], and the (offset, length) pairs of the
+    // seq and qual fields that start in it in bam_fields[bam_fcur], their offsets also on the host (bam_field_off).  The
+    // other buffer of each pair takes the carried rest when the stream is compressed.
+    DevBuf bam_buf[2], bam_fields[2], bam_recs, bam_pos, bam_text, bam_hfields;
+    int bam_cur = 0, bam_fcur = 0;
+    int64_t bam_base = 0, bam_len = 0;
+    std::vector<int64_t> bam_field_off;
+    // the records of the last bb_bam_build: stream offset and size of each (bam_last_at < 0: taken off the stream)
+    int64_t bam_last_at = -1;
+    std::vector<int64_t> bam_last_pos, bam_last_size;
+    uint8_t *h_bam = nullptr;   // pinned staging of bb_bam_fetch_records
+    int64_t h_bam_cap = 0;
+
     Worker &w0() { return *workers[0]; }
     ~bb_ctx() {
         for (cudaEvent_t e : {ev_t0, ev_t1}) if (e) cudaEventDestroy(e);
         if (bgzf_stream) cudaStreamDestroy(bgzf_stream);
         if (h_bgzf) cudaFreeHost(h_bgzf);
+        if (h_bam) cudaFreeHost(h_bam);
     }
 };
 
@@ -1031,6 +1049,15 @@ extern "C" int64_t bb_bgzf_bound(int64_t n) {
 // against 34 ms with 2048.
 constexpr int64_t kBgzfPassChunks = 2048;
 
+// The compressor's stream and the pinned words its passes report through (created by the first call that needs them).
+static int ensure_bgzf_stream(bb_ctx *ctx) {
+    if (!ctx->bgzf_stream) {
+        BB_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->bgzf_stream, cudaStreamNonBlocking));
+        BB_CUDA(ctx, cudaHostAlloc((void **)&ctx->h_bgzf, 2 * sizeof(int64_t), cudaHostAllocPortable));
+    }
+    return BB_OK;
+}
+
 extern "C" int bb_bgzf_compress(bb_ctx *ctx, const uint8_t *in, int64_t n, int line_mod4, int final, uint8_t *out,
                                 int64_t out_cap, int64_t *n_out, int64_t *n_consumed) {
     if (!ctx || n < 0 || (n && !in) || line_mod4 < 0 || line_mod4 > 3 || out_cap < 0 || !n_out || !n_consumed)
@@ -1043,10 +1070,7 @@ extern "C" int bb_bgzf_compress(bb_ctx *ctx, const uint8_t *in, int64_t n, int l
         return set_err(ctx, BB_ERR_CAPACITY, "bb_bgzf_compress: out_cap is less than bb_bgzf_bound of the input");
     }
     BB_CUDA(ctx, cudaSetDevice(ctx->device));
-    if (!ctx->bgzf_stream) {
-        BB_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->bgzf_stream, cudaStreamNonBlocking));
-        BB_CUDA(ctx, cudaHostAlloc((void **)&ctx->h_bgzf, 2 * sizeof(int64_t), cudaHostAllocPortable));
-    }
+    if (const int rc = ensure_bgzf_stream(ctx)) return rc;
     const cudaStream_t st = ctx->bgzf_stream;
     int mod4 = line_mod4;
     int64_t done = 0, written = 0;
@@ -1125,6 +1149,7 @@ extern "C" int bb_batch_upload(bb_ctx *ctx, int32_t n_reads, const uint64_t *rea
     if (n_reads <= 0 || !read_index || !seg_off || !segs || !target_identity || literal_len < 0)
         return set_err(ctx, BB_ERR_ARG, "bb_batch_upload: bad arguments");
     if (!ctx->have_em || !ctx->have_qm) return set_err(ctx, BB_ERR_STATE, "upload the error and qscore models first");
+    ctx->fetched = false;   // the workers' output buffers are about to be reused
     std::vector<int64_t> len;
     if (const int rc = check_batch(ctx, n_reads, seg_off, segs, literal_len, len)) return rc;
     const int n_workers = (int)ctx->workers.size();
@@ -1188,6 +1213,7 @@ extern "C" int bb_batch_upload(bb_ctx *ctx, int32_t n_reads, const uint64_t *rea
 // Asynchronous: the kernel chains of all workers are enqueued from this thread and overlap on the device.
 extern "C" int bb_batch_run(bb_ctx *ctx) {
     if (!ctx) return BB_ERR_ARG;
+    ctx->fetched = false;   // the run rewrites the workers' output buffers
     BB_CUDA(ctx, cudaSetDevice(ctx->device));
     const cudaStream_t st0 = ctx->w0().stream;
     BB_CUDA(ctx, cudaEventRecord(ctx->ev_t0, st0));
@@ -1306,8 +1332,10 @@ extern "C" int bb_trace_dump(bb_ctx *ctx, const char *path) {
 
 // Finishes every worker's run, packs their blocks back to back in the caller's buffers and fills the results.
 // eager: the copies of a worker were already enqueued behind its kernels with these bases (bb_sequence_batch).
+// Without `copy` the blocks stay on the device (bb_fetch_last_batch_results).
 static int fetch_all(bb_ctx *ctx, bb_read_result *results, uint8_t *seq_out, uint8_t *qual_out, int64_t out_cap,
-                     int64_t *out_total, const std::vector<int64_t> *eager_bases) {
+                     int64_t *out_total, const std::vector<int64_t> *eager_bases, bool copy = true) {
+    ctx->fetched = false;
     std::vector<int64_t> base((size_t)ctx->n_split, 0);
     int64_t total = 0;
     bool moved = false;  // a worker's output size changed after the eager copies were placed (it had to run again)
@@ -1321,16 +1349,29 @@ static int fetch_all(bb_ctx *ctx, bb_read_result *results, uint8_t *seq_out, uin
     });
     if (rc) return rc;
     if (out_total) *out_total = total;
-    if (out_cap < total) return set_err(ctx, BB_ERR_CAPACITY, "output buffers too small");
-    if (total && (!seq_out || !qual_out)) return set_err(ctx, BB_ERR_ARG, "null output buffers");
-    const bool have_eager = eager_bases && !moved && *eager_bases == base;
-    if (!have_eager && (rc = each_worker(ctx, [&](Worker &w, int i) -> int { return w_copy_out(w, base[(size_t)i], seq_out, qual_out); })))
-        return rc;
-    return each_worker(ctx, [&](Worker &w, int i) -> int {
+    if (copy) {
+        if (out_cap < total) return set_err(ctx, BB_ERR_CAPACITY, "output buffers too small");
+        if (total && (!seq_out || !qual_out)) return set_err(ctx, BB_ERR_ARG, "null output buffers");
+        const bool have_eager = eager_bases && !moved && *eager_bases == base;
+        if (!have_eager && (rc = each_worker(ctx, [&](Worker &w, int i) -> int { return w_copy_out(w, base[(size_t)i], seq_out, qual_out); })))
+            return rc;
+    }
+    rc = each_worker(ctx, [&](Worker &w, int i) -> int {
         BB_CUDA(&w, cudaSetDevice(ctx->device));
         BB_CUDA(&w, cudaStreamSynchronize(w.stream));
         return w_results(w, results, ctx->n_split == 1 ? nullptr : ctx->part[(size_t)i].data(), base[(size_t)i]);
     });
+    if (rc) return rc;
+    ctx->out_base = base;
+    ctx->out_base.push_back(total);
+    ctx->fetched = true;
+    return BB_OK;
+}
+
+extern "C" int bb_fetch_last_batch_results(bb_ctx *ctx, bb_read_result *results, int64_t *out_total) {
+    if (!ctx) return BB_ERR_ARG;
+    if (!results) return set_err(ctx, BB_ERR_ARG, "bb_fetch_last_batch_results: bad arguments");
+    return fetch_all(ctx, results, nullptr, nullptr, 0, out_total, nullptr, false);
 }
 
 extern "C" int bb_fetch_last_batch(bb_ctx *ctx, bb_read_result *results, uint8_t *seq_out, uint8_t *qual_out,
@@ -1363,6 +1404,215 @@ extern "C" int bb_sequence_batch(bb_ctx *ctx, int32_t n_reads, const uint64_t *r
         if ((rc = w_copy_out(wk, base[(size_t)w], seq_out, qual_out))) { eager = false; break; }
     }
     return fetch_all(ctx, results, seq_out, qual_out, out_cap, out_total, eager ? &base : nullptr);
+}
+
+// ---- BAM output: records built on the device, compressed by the BGZF compressor --------------------------
+// Passes of bgzf_k_compress_bam over use bytes of a record stream starting at byte stream_base: from the device buffer
+// d_in, or from host memory h_in (then copied to bgzf_in pass by pass).  Members to out (capacity checked by the caller).
+static int bam_passes(bb_ctx *ctx, const uint8_t *h_in, const uint8_t *d_in, int64_t use, int64_t stream_base,
+                      const int64_t *d_fields, int64_t n_fields, uint8_t *out, int64_t *n_out) {
+    const cudaStream_t st = ctx->bgzf_stream;
+    int64_t done = 0, written = 0;
+    while (done < use) {
+        const int64_t len = std::min(use - done, kBgzfPassChunks * BB_BGZF_CHUNK);
+        const int nc = (int)((len + BB_BGZF_CHUNK - 1) / BB_BGZF_CHUNK);
+        BB_CUDA(ctx, ctx->bgzf_slots.ensure((size_t)nc * 65536));
+        BB_CUDA(ctx, ctx->bgzf_sizes.ensure((size_t)nc * sizeof(int32_t)));
+        BB_CUDA(ctx, ctx->bgzf_off.ensure((size_t)(nc + 1) * sizeof(int64_t)));
+        BB_CUDA(ctx, ctx->bgzf_out.ensure((size_t)bb_bgzf_bound(len)));
+        const uint8_t *src = d_in ? d_in + done : nullptr;
+        if (!src) {
+            BB_CUDA(ctx, ctx->bgzf_in.ensure((size_t)len));
+            BB_CUDA(ctx, cudaMemcpyAsync(ctx->bgzf_in.p, h_in + done, (size_t)len, cudaMemcpyHostToDevice, st));
+            src = ctx->bgzf_in.as<uint8_t>();
+        }
+        bbl_bgzf_pass_bam(st, src, len, nc, d_fields, n_fields, stream_base + done, ctx->bgzf_slots.as<uint8_t>(),
+                          ctx->bgzf_sizes.as<int32_t>(), ctx->bgzf_off.as<int64_t>(), ctx->bgzf_out.as<uint8_t>());
+        BB_CUDA(ctx, cudaGetLastError());
+        BB_CUDA(ctx, cudaMemcpyAsync(ctx->h_bgzf + 1, ctx->bgzf_off.as<int64_t>() + nc, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+        BB_CUDA(ctx, cudaStreamSynchronize(st));
+        const int64_t bytes = ctx->h_bgzf[1];
+        if (bytes <= 0 || bytes > bb_bgzf_bound(len))
+            return set_err(ctx, BB_ERR_INTERNAL, "BAM compressor: members of " + std::to_string(bytes) + " bytes");
+        BB_CUDA(ctx, cudaMemcpyAsync(out + written, ctx->bgzf_out.p, (size_t)bytes, cudaMemcpyDeviceToHost, st));
+        BB_CUDA(ctx, cudaStreamSynchronize(st));
+        written += bytes;
+        done += len;
+    }
+    *n_out = written;
+    return BB_OK;
+}
+
+// Makes the current buffer of `pair` (index cur) hold at least `bytes`: when it is too small, its first `keep` bytes move
+// to the other buffer, which becomes the current one.
+static int grow_keep(bb_ctx *ctx, DevBuf (&pair)[2], int &cur, size_t bytes, size_t keep) {
+    if (bytes <= pair[cur].cap) return BB_OK;
+    BB_CUDA(ctx, pair[1 - cur].ensure(bytes));
+    if (keep) BB_CUDA(ctx, cudaMemcpyAsync(pair[1 - cur].p, pair[cur].p, keep, cudaMemcpyDeviceToDevice, ctx->bgzf_stream));
+    BB_CUDA(ctx, cudaStreamSynchronize(ctx->bgzf_stream));
+    pair[cur].release();
+    cur = 1 - cur;
+    return BB_OK;
+}
+
+extern "C" int bb_bam_build(bb_ctx *ctx, int32_t n, const bb_bam_record *recs, const uint8_t *text, int64_t text_len) {
+    if (!ctx) return BB_ERR_ARG;
+    if (n < 0 || (n && !recs) || text_len < 0 || (text_len && !text)) return set_err(ctx, BB_ERR_ARG, "bb_bam_build: bad arguments");
+    if (!ctx->fetched) return set_err(ctx, BB_ERR_STATE, "bb_bam_build: no fetched batch (bb_fetch_last_batch_results)");
+    const std::vector<int64_t> &base = ctx->out_base;
+    const int n_src = (int)base.size() - 1;
+    std::vector<int64_t> pos((size_t)n), size((size_t)n);
+    int64_t at = ctx->bam_len;
+    for (int32_t i = 0; i < n; i++) {
+        const bb_bam_record &r = recs[i];
+        int k = 0;
+        while (k + 1 < n_src && r.out_off >= base[(size_t)k + 1]) k++;
+        if (r.out_off < 0 || r.out_len < 0 || r.out_off + r.out_len > base[(size_t)k + 1] || r.name_len < 0 || r.name_len > 254 ||
+            r.co_len < 0 || r.text_off < 0 || r.text_off + r.name_len + r.co_len > text_len) {
+            char msg[160];
+            std::snprintf(msg, sizeof(msg), "bb_bam_build: record %d lies outside the batch output or the text", i);
+            return set_err(ctx, BB_ERR_ARG, msg);
+        }
+        pos[(size_t)i] = at;
+        size[(size_t)i] = bbl_bam_record_size(r.name_len, r.out_len, r.co_len);
+        at += size[(size_t)i];
+    }
+    BB_CUDA(ctx, cudaSetDevice(ctx->device));
+    if (int rc = ensure_bgzf_stream(ctx)) return rc;
+    const cudaStream_t st = ctx->bgzf_stream;
+    const size_t nf = ctx->bam_field_off.size();
+    if (int rc = grow_keep(ctx, ctx->bam_buf, ctx->bam_cur, (size_t)std::max<int64_t>(at, 1), (size_t)ctx->bam_len)) return rc;
+    if (int rc = grow_keep(ctx, ctx->bam_fields, ctx->bam_fcur, (nf + 2 * (size_t)n + 1) * 2 * sizeof(int64_t),
+                           nf * 2 * sizeof(int64_t)))
+        return rc;
+    if (n > 0) {
+        int rc;
+        if ((rc = upload(ctx, st, ctx->bam_recs, recs, (size_t)n))) return rc;
+        if ((rc = upload(ctx, st, ctx->bam_pos, pos.data(), (size_t)n))) return rc;
+        if ((rc = upload(ctx, st, ctx->bam_text, text, (size_t)text_len))) return rc;
+        std::vector<const uint8_t *> seq((size_t)n_src), qual((size_t)n_src);
+        for (int k = 0; k < n_src; k++) {
+            seq[(size_t)k] = ctx->workers[(size_t)k]->d_out_seq.as<uint8_t>();
+            qual[(size_t)k] = ctx->workers[(size_t)k]->d_out_qual.as<uint8_t>();
+        }
+        bbl_bam_records(st, n, ctx->bam_recs.as<bb_bam_record>(), ctx->bam_pos.as<int64_t>(), ctx->bam_text.as<uint8_t>(), n_src,
+                        seq.data(), qual.data(), base.data(), ctx->bam_buf[ctx->bam_cur].as<uint8_t>(), ctx->bam_base,
+                        ctx->bam_fields[ctx->bam_fcur].as<int64_t>() + 2 * nf);
+        BB_CUDA(ctx, cudaGetLastError());
+    }
+    BB_CUDA(ctx, cudaStreamSynchronize(st));
+    ctx->bam_last_at = ctx->bam_base + ctx->bam_len;
+    ctx->bam_last_pos.assign(pos.begin(), pos.end());
+    ctx->bam_last_size.assign(size.begin(), size.end());
+    for (int32_t i = 0; i < n; i++) {
+        const int64_t o_seq = ctx->bam_base + pos[(size_t)i] + 36 + recs[i].name_len + 1;
+        ctx->bam_field_off.push_back(o_seq);
+        ctx->bam_field_off.push_back(o_seq + (recs[i].out_len + 1) / 2);
+    }
+    ctx->bam_len = at;
+    return BB_OK;
+}
+
+extern "C" int bb_bam_compress_device(bb_ctx *ctx, int final, uint8_t *out, int64_t out_cap, int64_t *n_out) {
+    if (!ctx) return BB_ERR_ARG;
+    if (out_cap < 0 || !n_out) return set_err(ctx, BB_ERR_ARG, "bb_bam_compress_device: bad arguments");
+    const int64_t use = final ? ctx->bam_len : ctx->bam_len / BB_BGZF_CHUNK * BB_BGZF_CHUNK;
+    *n_out = 0;
+    if (bb_bgzf_bound(use) > out_cap || (use && !out)) {
+        *n_out = bb_bgzf_bound(use);
+        return set_err(ctx, BB_ERR_CAPACITY, "bb_bam_compress_device: out_cap is less than bb_bgzf_bound of the input");
+    }
+    if (!use) return BB_OK;
+    BB_CUDA(ctx, cudaSetDevice(ctx->device));
+    if (int rc = ensure_bgzf_stream(ctx)) return rc;
+    const int cur = ctx->bam_cur, fcur = ctx->bam_fcur;
+    const int64_t nf = (int64_t)ctx->bam_field_off.size();
+    if (int rc = bam_passes(ctx, nullptr, ctx->bam_buf[cur].as<uint8_t>(), use, ctx->bam_base, ctx->bam_fields[fcur].as<int64_t>(),
+                            nf, out, n_out))
+        return rc;
+    // the rest (less than a chunk) and the fields that start in it move to the front of the other buffers
+    const int64_t rest = ctx->bam_len - use, new_base = ctx->bam_base + use;
+    const int64_t keep_from = std::upper_bound(ctx->bam_field_off.begin(), ctx->bam_field_off.end(), new_base) -
+                              ctx->bam_field_off.begin();
+    const int64_t nk = nf - keep_from;
+    BB_CUDA(ctx, ctx->bam_buf[1 - cur].ensure((size_t)std::max<int64_t>(rest, 1)));
+    BB_CUDA(ctx, ctx->bam_fields[1 - fcur].ensure((size_t)std::max<int64_t>(nk, 1) * 2 * sizeof(int64_t)));
+    if (rest) BB_CUDA(ctx, cudaMemcpyAsync(ctx->bam_buf[1 - cur].p, ctx->bam_buf[cur].as<uint8_t>() + use, (size_t)rest,
+                                           cudaMemcpyDeviceToDevice, ctx->bgzf_stream));
+    if (nk) BB_CUDA(ctx, cudaMemcpyAsync(ctx->bam_fields[1 - fcur].p, ctx->bam_fields[fcur].as<int64_t>() + 2 * keep_from,
+                                         (size_t)nk * 2 * sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->bgzf_stream));
+    BB_CUDA(ctx, cudaStreamSynchronize(ctx->bgzf_stream));
+    ctx->bam_cur = 1 - cur;
+    ctx->bam_fcur = 1 - fcur;
+    ctx->bam_field_off.erase(ctx->bam_field_off.begin(), ctx->bam_field_off.begin() + keep_from);
+    ctx->bam_base = new_base;
+    ctx->bam_len = rest;
+    ctx->bam_last_at = -1;
+    return BB_OK;
+}
+
+extern "C" int bb_bam_fetch_records(bb_ctx *ctx, const int64_t *dst_off, uint8_t *out, int64_t out_cap, int64_t *n_bytes) {
+    if (!ctx) return BB_ERR_ARG;
+    if (!n_bytes || out_cap < 0) return set_err(ctx, BB_ERR_ARG, "bb_bam_fetch_records: bad arguments");
+    *n_bytes = 0;
+    if (ctx->bam_last_at < 0) return set_err(ctx, BB_ERR_STATE, "bb_bam_fetch_records: no records built since the stream was last compressed or fetched");
+    const int64_t from = ctx->bam_last_at - ctx->bam_base, bytes = ctx->bam_len - from;
+    const size_t n = ctx->bam_last_pos.size();
+    *n_bytes = bytes;
+    if (bytes && !out) return set_err(ctx, BB_ERR_ARG, "bb_bam_fetch_records: bad arguments");
+    for (size_t i = 0; i < n; i++) {
+        const int64_t to = dst_off ? dst_off[i] : ctx->bam_last_pos[i] - from;
+        if (to < 0 || to + ctx->bam_last_size[i] > out_cap)
+            return set_err(ctx, BB_ERR_CAPACITY, "bb_bam_fetch_records: record " + std::to_string(i) + " does not fit out_cap");
+    }
+    BB_CUDA(ctx, cudaSetDevice(ctx->device));
+    if (bytes > ctx->h_bam_cap) {
+        if (ctx->h_bam) cudaFreeHost(ctx->h_bam);
+        ctx->h_bam = nullptr;
+        ctx->h_bam_cap = 0;
+        BB_CUDA(ctx, cudaHostAlloc((void **)&ctx->h_bam, (size_t)(bytes + bytes / 4), cudaHostAllocPortable));
+        ctx->h_bam_cap = bytes + bytes / 4;
+    }
+    if (bytes) {
+        BB_CUDA(ctx, cudaMemcpyAsync(ctx->h_bam, ctx->bam_buf[ctx->bam_cur].as<uint8_t>() + from, (size_t)bytes,
+                                     cudaMemcpyDeviceToHost, ctx->bgzf_stream));
+        BB_CUDA(ctx, cudaStreamSynchronize(ctx->bgzf_stream));
+    }
+    for (size_t i = 0; i < n; i++) {
+        const int64_t at = ctx->bam_last_pos[i] - from;
+        std::memcpy(out + (dst_off ? dst_off[i] : at), ctx->h_bam + at, (size_t)ctx->bam_last_size[i]);
+    }
+    ctx->bam_len = from;
+    ctx->bam_field_off.resize(ctx->bam_field_off.size() - 2 * n);
+    ctx->bam_last_at = -1;
+    return BB_OK;
+}
+
+extern "C" int bb_bam_compress(bb_ctx *ctx, const uint8_t *in, int64_t n, int64_t stream_base, const int64_t *fields,
+                               int64_t n_fields, int final, uint8_t *out, int64_t out_cap, int64_t *n_out, int64_t *n_consumed) {
+    if (!ctx) return BB_ERR_ARG;
+    if (n < 0 || (n && !in) || stream_base < 0 || n_fields < 0 || (n_fields && !fields) || out_cap < 0 || !n_out || !n_consumed)
+        return set_err(ctx, BB_ERR_ARG, "bb_bam_compress: bad arguments");
+    for (int64_t i = 0; i < n_fields; i++)   // block starts must come in order, at least a field apart
+        if (fields[2 * i + 1] < 0 || (i && fields[2 * i - 2] + fields[2 * i - 1] > fields[2 * i]))
+            return set_err(ctx, BB_ERR_ARG, "bb_bam_compress: fields overlap or are out of order");
+    const int64_t use = final ? n : n / BB_BGZF_CHUNK * BB_BGZF_CHUNK;
+    *n_out = 0;
+    *n_consumed = 0;
+    if (bb_bgzf_bound(use) > out_cap || (use && !out)) {
+        *n_out = bb_bgzf_bound(use);
+        return set_err(ctx, BB_ERR_CAPACITY, "bb_bam_compress: out_cap is less than bb_bgzf_bound of the input");
+    }
+    if (!use) return BB_OK;
+    BB_CUDA(ctx, cudaSetDevice(ctx->device));
+    if (int rc = ensure_bgzf_stream(ctx)) return rc;
+    int64_t f0 = 0, f1 = n_fields;   // the fields that start inside in[0 .. use)
+    while (f0 < n_fields && fields[2 * f0] < stream_base) f0++;
+    while (f1 > f0 && fields[2 * (f1 - 1)] >= stream_base + use) f1--;
+    if (int rc = upload(ctx, ctx->bgzf_stream, ctx->bam_hfields, fields + 2 * f0, (size_t)(f1 - f0) * 2)) return rc;
+    if (int rc = bam_passes(ctx, in, nullptr, use, stream_base, ctx->bam_hfields.as<int64_t>(), f1 - f0, out, n_out)) return rc;
+    *n_consumed = use;
+    return BB_OK;
 }
 
 // ---- single-pair entry points (worker 0's stream and scratch) ----------------------------------------------

@@ -12,6 +12,10 @@
 // Chunks sit at fixed offsets of the whole stream (the caller carries the tail between calls), so the compressed
 // bytes do not depend on where the caller's buffers end.  Everything a CTA computes is a function of its chunk and
 // the index mod 4 of the FASTQ line its first byte belongs to: the output is deterministic.
+//
+// BAM records (bgzf_k_compress_bam) are segmented the same way without a newline scan: a block starts at every seq or
+// qual field (bb_bam_out.cuh) that starts after the chunk's first byte and has at least BGZF_MIN_SEG bytes in the chunk;
+// the fixed fields, name and CO tag of a record stay in the block of the qual field before them.
 #pragma once
 #ifndef BB_EMULATOR
 #include <cuda_runtime.h>
@@ -249,12 +253,12 @@ __device__ void bgzf_write_header(BGZFSmem &s, uint32_t pos, int final, int hcle
     }
 }
 
-// One CTA per chunk: chunk c is in[c * BGZF_CHUNK .. min(n, (c + 1) * BGZF_CHUNK)), its first byte on a line whose
-// index mod 4 is line_pref[c] & 3.  Writes the member to slots[c * BGZF_SLOT ..] (whole words) and its size to sizes[c].
-// Dynamic shared memory: BGZF_SMEM_BYTES.
-__global__ void __launch_bounds__(BGZF_THREADS, 1)
-bgzf_k_compress(const uint8_t *__restrict__ in, int64_t n, const int64_t *__restrict__ line_pref, uint8_t *__restrict__ slots,
-                int32_t *__restrict__ sizes) {
+// Chunk c of in[0..n) into its member; the body of both compressor kernels.  kBam selects where the deflate blocks start:
+// FASTQ lines found by a newline scan (line_pref), or the seq and qual fields of BAM records (fields, stream_base).
+template <bool kBam>
+__device__ __forceinline__ void bgzf_compress_chunk(const uint8_t *__restrict__ in, int64_t n, const int64_t *__restrict__ line_pref,
+                                                    const int64_t *__restrict__ fields, int64_t n_fields, int64_t stream_base,
+                                                    uint8_t *__restrict__ slots, int32_t *__restrict__ sizes) {
 #ifdef BB_EMULATOR
     static BGZFSmem s_mem;
     BGZFSmem &s = s_mem;
@@ -266,7 +270,8 @@ bgzf_k_compress(const uint8_t *__restrict__ in, int64_t n, const int64_t *__rest
     const int64_t c = blockIdx.x;
     const int64_t base = c * BGZF_CHUNK;
     const int len = (int)(n - base < BGZF_CHUNK ? n - base : BGZF_CHUNK);
-    const int mod4 = (int)(line_pref[c] & 3);
+    int mod4 = 0;
+    if constexpr (!kBam) mod4 = (int)(line_pref[c] & 3);
     const uint8_t *src = in + base;
     {   // chunk and CRC table into shared memory, member buffer cleared
         const int n16 = len >> 4;
@@ -283,35 +288,71 @@ bgzf_k_compress(const uint8_t *__restrict__ in, int64_t n, const int64_t *__rest
     uint32_t nl = 0, crc = 0;
     for (int i = a0; i < a1; i++) {
         const uint8_t b = s.in[i];
-        nl += b == '\n';
+        if constexpr (!kBam) nl += b == '\n';
         crc = s.crc_table[(crc ^ b) & 0xffu] ^ (crc >> 8);
     }
-    uint32_t nl_all;
-    const uint32_t nl_before = bgzf_scan(s, nl, &nl_all);
+    uint32_t nl_before = 0;
+    if constexpr (!kBam) {
+        uint32_t nl_all;
+        nl_before = bgzf_scan(s, nl, &nl_all);
+    }
     // CRC-32 of the chunk = the slices' registers moved past the bytes after them, and the initial register past all
     uint32_t term = a1 > a0 ? bgzf_mulmod(crc, bgzf_x8n((uint32_t)(len - a1))) : 0u;
     for (int d = 16; d > 0; d >>= 1) term ^= __shfl_xor_sync(0xffffffffu, term, d);
     if ((t & 31) == 0) s.crc_part[t >> 5] = term;
 
-    // block starts: sequence (line index 1 mod 4) and quality (3 mod 4) lines with BGZF_MIN_SEG bytes in the chunk
-    uint32_t n_starts = 0;
-    for (int pass = 0; pass < 2; pass++) {
-        uint32_t at = 0;
-        if (pass) {
-            uint32_t all;
-            at = 1 + bgzf_scan(s, n_starts, &all);
-            if (t == 0) { s.blk_start[0] = 0; s.n_blocks = 1 + (int)all; s.blk_start[1 + all] = len; }
+    if constexpr (kBam) {
+        // block starts: seq and qual fields that start after the chunk's first byte with BGZF_MIN_SEG bytes in the chunk
+        // (fields: (stream offset, length) pairs in stream order; in[0] is byte stream_base of the record stream)
+        const int64_t cs = stream_base + base, last = cs + len - BGZF_MIN_SEG;
+        int64_t lo = 0, hi = n_fields;
+        while (lo < hi) {   // first field that starts after cs
+            const int64_t mid = (lo + hi) >> 1;
+            if (fields[2 * mid] > cs) hi = mid; else lo = mid + 1;
         }
-        uint32_t line = (uint32_t)mod4 + nl_before;
-        for (int i = a0; i < a1; i++) {
-            if (i > a0 && s.in[i - 1] == '\n') line++;
-            if (i > 0 && s.in[i - 1] == '\n') {
-                if ((line & 1u) && i + BGZF_MIN_SEG <= len) {
-                    int j = i;
-                    while (j < i + BGZF_MIN_SEG - 1 && s.in[j] != '\n') j++;
-                    if (j == i + BGZF_MIN_SEG - 1) {
-                        if (pass) s.blk_start[at++] = i;
-                        else n_starts++;
+        const int64_t f0 = lo;
+        hi = n_fields;
+        while (lo < hi) {   // first field that starts after last
+            const int64_t mid = (lo + hi) >> 1;
+            if (fields[2 * mid] > last) hi = mid; else lo = mid + 1;
+        }
+        const int64_t nf = lo - f0, fper = (nf + BGZF_THREADS - 1) / BGZF_THREADS;
+        const int64_t g0 = f0 + min((int64_t)t * fper, nf), g1 = f0 + min((int64_t)t * fper + fper, nf);
+        uint32_t n_starts = 0;
+        for (int pass = 0; pass < 2; pass++) {
+            uint32_t at = 0;
+            if (pass) {
+                uint32_t all;
+                at = 1 + bgzf_scan(s, n_starts, &all);
+                if (t == 0) { s.blk_start[0] = 0; s.n_blocks = 1 + (int)all; s.blk_start[1 + all] = len; }
+            }
+            for (int64_t g = g0; g < g1; g++)
+                if (fields[2 * g + 1] >= BGZF_MIN_SEG) {
+                    if (pass) s.blk_start[at++] = (int)(fields[2 * g] - cs);
+                    else n_starts++;
+                }
+        }
+    } else {
+        // block starts: sequence (line index 1 mod 4) and quality (3 mod 4) lines with BGZF_MIN_SEG bytes in the chunk
+        uint32_t n_starts = 0;
+        for (int pass = 0; pass < 2; pass++) {
+            uint32_t at = 0;
+            if (pass) {
+                uint32_t all;
+                at = 1 + bgzf_scan(s, n_starts, &all);
+                if (t == 0) { s.blk_start[0] = 0; s.n_blocks = 1 + (int)all; s.blk_start[1 + all] = len; }
+            }
+            uint32_t line = (uint32_t)mod4 + nl_before;
+            for (int i = a0; i < a1; i++) {
+                if (i > a0 && s.in[i - 1] == '\n') line++;
+                if (i > 0 && s.in[i - 1] == '\n') {
+                    if ((line & 1u) && i + BGZF_MIN_SEG <= len) {
+                        int j = i;
+                        while (j < i + BGZF_MIN_SEG - 1 && s.in[j] != '\n') j++;
+                        if (j == i + BGZF_MIN_SEG - 1) {
+                            if (pass) s.blk_start[at++] = i;
+                            else n_starts++;
+                        }
                     }
                 }
             }
@@ -403,6 +444,23 @@ bgzf_k_compress(const uint8_t *__restrict__ in, int64_t n, const int64_t *__rest
     __syncthreads();
     uint32_t *dst = reinterpret_cast<uint32_t *>(slots + c * BGZF_SLOT);
     for (uint32_t i = t; i < (size + 3) / 4; i += BGZF_THREADS) dst[i] = s.out[i];
+}
+
+// One CTA per chunk: chunk c is in[c * BGZF_CHUNK .. min(n, (c + 1) * BGZF_CHUNK)), its first byte on a line whose
+// index mod 4 is line_pref[c] & 3.  Writes the member to slots[c * BGZF_SLOT ..] (whole words) and its size to sizes[c].
+// Dynamic shared memory: BGZF_SMEM_BYTES.
+__global__ void __launch_bounds__(BGZF_THREADS, 1)
+bgzf_k_compress(const uint8_t *__restrict__ in, int64_t n, const int64_t *__restrict__ line_pref, uint8_t *__restrict__ slots,
+                int32_t *__restrict__ sizes) {
+    bgzf_compress_chunk<false>(in, n, line_pref, nullptr, 0, 0, slots, sizes);
+}
+
+// The same for a stream of BAM records whose byte in[0] is byte stream_base of the stream: deflate blocks start at the
+// seq and qual fields listed in fields[2 * n_fields] as (stream offset, length) pairs in stream order (bb_bam_out.cuh).
+__global__ void __launch_bounds__(BGZF_THREADS, 1)
+bgzf_k_compress_bam(const uint8_t *__restrict__ in, int64_t n, const int64_t *__restrict__ fields, int64_t n_fields,
+                    int64_t stream_base, uint8_t *__restrict__ slots, int32_t *__restrict__ sizes) {
+    bgzf_compress_chunk<true>(in, n, nullptr, fields, n_fields, stream_base, slots, sizes);
 }
 
 // Newlines of every chunk (one CTA each) -> counts[c].

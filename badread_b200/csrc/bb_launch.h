@@ -42,3 +42,15 @@ void bbl_align_pair(cudaStream_t st, const uint8_t *q, int n, const uint8_t *t, 
 cudaError_t bbl_bgzf_init();
 void bbl_bgzf_pass(cudaStream_t st, const uint8_t *in, int64_t n, int n_chunks, int line_mod4, int32_t *lines,
                    int64_t *line_pref, uint8_t *slots, int32_t *sizes, int64_t *offsets, uint8_t *out);
+// The same for BAM records: in[0] is byte stream_base of the record stream, fields[2 * n_fields] the (stream offset,
+// length) pairs of the seq and qual fields in stream order (no newline scan).
+void bbl_bgzf_pass_bam(cudaStream_t st, const uint8_t *in, int64_t n, int n_chunks, const int64_t *fields, int64_t n_fields,
+                       int64_t stream_base, uint8_t *slots, int32_t *sizes, int64_t *offsets, uint8_t *out);
+// BAM records (bb_bam_out.cuh): record i of recs[n_records] to out[pos[i] ..], its bases and qualities read from the n_src
+// output buffers seq[k] / qual[k] holding bytes [src_base[k], src_base[k + 1]) of the batch output; fields[4 i ..] = stream
+// offset and length of its seq and its qual field, out[0] being byte stream_base of the record stream.
+struct bb_bam_record;
+int64_t bbl_bam_record_size(int32_t name_len, int32_t l_seq, int32_t co_len);
+void bbl_bam_records(cudaStream_t st, int n_records, const bb_bam_record *recs, const int64_t *pos, const uint8_t *text,
+                     int n_src, const uint8_t *const *seq, const uint8_t *const *qual, const int64_t *src_base, uint8_t *out,
+                     int64_t stream_base, int64_t *fields);

@@ -595,16 +595,16 @@ extern "C" int bb_planner_view(const bb_planner *P, bb_plan_view *v) {
 }
 
 // ------------------------------------------------------------------------------------------------ FASTQ
-// simulate.py:70-86 for reads [first, n) of a finished batch, in read-index order: empty reads are skipped, a record is
-// "@{uuid} {info} length={len} error-free_length={frag} read_identity={100*matches/columns:.3f}%\n{seq}\n+\n{qual}\n",
-// and the loop stops once the running total of emitted bases reaches the target.  With n_shards > 1 the batch was
-// dealt out over that many contexts (GPUs): read j of the batch is read j / n_shards of shard j % n_shards.
-extern "C" int bb_fastq_format_sharded(int32_t n_shards, const bb_plan_view *const *views,
-                                       const bb_read_result *const *results, const uint8_t *const *seq,
-                                       const uint8_t *const *qual, int32_t first, int64_t bases_so_far,
-                                       int64_t target_bases, int32_t n_threads, uint8_t *out, int64_t out_cap,
-                                       int64_t *out_len, int32_t *n_emitted, int64_t *bases_emitted, int32_t *next_read) {
-    if (n_shards <= 0 || !views || !results || !out_len || first < 0) return BB_ERR_ARG;
+namespace {
+
+struct Emitted { int32_t g, i; };
+
+// simulate.py:63-70 for reads [first, n) of a finished batch dealt out over n_shards contexts (read j of the batch is read
+// j / n_shards of shard j % n_shards), in read-index order: empty reads are skipped, and the loop stops once the running
+// total of emitted bases reaches the target.  *next_j = the first read not consumed, *total = the running total.
+int select_emitted(int32_t n_shards, const bb_plan_view *const *views, const bb_read_result *const *results, int32_t first,
+                   int64_t bases_so_far, int64_t target_bases, std::vector<Emitted> &emit, int64_t *next_j, int64_t *total) {
+    if (n_shards <= 0 || !views || !results || first < 0) return BB_ERR_ARG;
     int64_t n = 0;
     for (int g = 0; g < n_shards; g++) {
         if (!views[g] || !results[g]) return BB_ERR_ARG;
@@ -612,21 +612,57 @@ extern "C" int bb_fastq_format_sharded(int32_t n_shards, const bb_plan_view *con
     }
     for (int g = 0; g < n_shards; g++)  // shard g must hold reads g, g + G, ...
         if (views[g]->n_reads != (n - g + n_shards - 1) / n_shards) return BB_ERR_ARG;
-    struct Rec { int32_t g, i; };
-    std::vector<Rec> emit;
-    int64_t total = bases_so_far;
+    int64_t sum = bases_so_far;
     int64_t j = first;
-    for (; j < n && total < target_bases; j++) {
+    for (; j < n && sum < target_bases; j++) {
         const int g = (int)(j % n_shards), i = (int)(j / n_shards);
         const bb_read_result &r = results[g][i];
         if (r.out_len <= 0) continue;
-        emit.push_back(Rec{g, i});
-        total += r.out_len;
+        emit.push_back(Emitted{g, i});
+        sum += r.out_len;
     }
-    const int64_t next_j = j;
+    *next_j = j;
+    *total = sum;
+    return BB_OK;
+}
+
+// The read's name: its UUID as uuid.UUID prints it (36 characters).
+void append_read_name(const bb_plan_view *v, int r, std::string &h) {
+    static const char hex[] = "0123456789abcdef";
+    const uint8_t *nm = v->read_names + (size_t)r * 16;
+    for (int b = 0; b < 16; b++) {
+        if (b == 4 || b == 6 || b == 8 || b == 10) h.push_back('-');
+        h.push_back(hex[nm[b] >> 4]); h.push_back(hex[nm[b] & 15]);
+    }
+}
+
+// The rest of the header line after the name and a space: "{info} length={len} error-free_length={frag}
+// read_identity={100*matches/columns:.3f}%" (simulate.py:73-75).
+void append_read_comment(const bb_plan_view *v, int r, const bb_read_result &rr, std::string &h) {
+    h.append(v->info + v->info_off[r], (size_t)(v->info_off[r + 1] - v->info_off[r]));
+    const double identity = rr.columns ? (double)rr.matches / (double)rr.columns : 0.0;
+    char buf[128];
+    std::snprintf(buf, sizeof(buf), " length=%d error-free_length=%d read_identity=%.3f%%", rr.out_len, rr.frag_len,
+                  identity * 100.0);
+    h += buf;
+}
+
+}  // namespace
+
+// simulate.py:70-86 for reads [first, n) of a finished batch, in read-index order (select_emitted): a record is
+// "@{uuid} {info} length={len} error-free_length={frag} read_identity={100*matches/columns:.3f}%\n{seq}\n+\n{qual}\n".
+extern "C" int bb_fastq_format_sharded(int32_t n_shards, const bb_plan_view *const *views,
+                                       const bb_read_result *const *results, const uint8_t *const *seq,
+                                       const uint8_t *const *qual, int32_t first, int64_t bases_so_far,
+                                       int64_t target_bases, int32_t n_threads, uint8_t *out, int64_t out_cap,
+                                       int64_t *out_len, int32_t *n_emitted, int64_t *bases_emitted, int32_t *next_read) {
+    if (!out_len) return BB_ERR_ARG;
+    std::vector<Emitted> emit;
+    int64_t next_j = 0, total = 0;
+    if (const int rc = select_emitted(n_shards, views, results, first, bases_so_far, target_bases, emit, &next_j, &total))
+        return rc;
     std::vector<std::string> headers(emit.size());
     std::vector<int64_t> off(emit.size() + 1, 0);
-    static const char hex[] = "0123456789abcdef";
     for (size_t e = 0; e < emit.size(); e++) {
         const bb_plan_view *v = views[emit[e].g];
         const int r = emit[e].i;
@@ -634,18 +670,10 @@ extern "C" int bb_fastq_format_sharded(int32_t n_shards, const bb_plan_view *con
         std::string &h = headers[e];
         h.reserve(160);
         h.push_back('@');
-        const uint8_t *nm = v->read_names + (size_t)r * 16;
-        for (int b = 0; b < 16; b++) {
-            if (b == 4 || b == 6 || b == 8 || b == 10) h.push_back('-');
-            h.push_back(hex[nm[b] >> 4]); h.push_back(hex[nm[b] & 15]);
-        }
+        append_read_name(v, r, h);
         h.push_back(' ');
-        h.append(v->info + v->info_off[r], (size_t)(v->info_off[r + 1] - v->info_off[r]));
-        const double identity = rr.columns ? (double)rr.matches / (double)rr.columns : 0.0;
-        char buf[128];
-        std::snprintf(buf, sizeof(buf), " length=%d error-free_length=%d read_identity=%.3f%%\n", rr.out_len, rr.frag_len,
-                      identity * 100.0);
-        h += buf;
+        append_read_comment(v, r, rr, h);
+        h.push_back('\n');
         off[e + 1] = off[e] + (int64_t)h.size() + 2ll * rr.out_len + 4;
     }
     const int64_t need = off[emit.size()];
@@ -680,7 +708,56 @@ extern "C" int bb_fastq_format_sharded(int32_t n_shards, const bb_plan_view *con
     return BB_OK;
 }
 
-extern "C" int bb_fastq_format(const bb_plan_view *v, const bb_read_result *results, const uint8_t *seq, const uint8_t *qual,
+// BAM records of the same emitted set (bb_bam_build builds them): the record sizes of bb_bam_out.cuh's bam_record_size.
+extern "C" int bb_bam_layout_sharded(int32_t n_shards, const bb_plan_view *const *views, const bb_read_result *const *results,
+                                     int32_t first, int64_t bases_so_far, int64_t target_bases, int64_t stream_base,
+                                     int32_t *shard, int32_t *index, int64_t *stream_off, bb_bam_record *recs, int64_t *fields,
+                                     uint8_t *text, int64_t text_cap, int64_t *text_len, int64_t *stream_len,
+                                     int32_t *n_emitted, int64_t *bases_emitted, int32_t *next_read) {
+    if (!text_len || !stream_len || stream_base < 0) return BB_ERR_ARG;
+    std::vector<Emitted> emit;
+    int64_t next_j = 0, total = 0;
+    if (const int rc = select_emitted(n_shards, views, results, first, bases_so_far, target_bases, emit, &next_j, &total))
+        return rc;
+    if (!emit.empty() && (!shard || !index || !stream_off || !recs || !fields)) return BB_ERR_ARG;
+    std::string all;
+    all.reserve(emit.size() * 160);
+    int64_t at = stream_base;
+    for (size_t e = 0; e < emit.size(); e++) {
+        const bb_plan_view *v = views[emit[e].g];
+        const int r = emit[e].i;
+        const bb_read_result &rr = results[emit[e].g][r];
+        bb_bam_record &o = recs[e];
+        o.out_off = rr.out_off;
+        o.out_len = rr.out_len;
+        o.text_off = (int64_t)all.size();
+        append_read_name(v, r, all);
+        o.name_len = (int32_t)((int64_t)all.size() - o.text_off);
+        append_read_comment(v, r, rr, all);
+        o.co_len = (int32_t)((int64_t)all.size() - o.text_off - o.name_len);
+        o.reserved = 0;
+        shard[e] = emit[e].g;
+        index[e] = r;
+        stream_off[e] = at;
+        const int64_t nb = ((int64_t)rr.out_len + 1) / 2;
+        const int64_t o_seq = at + 36 + o.name_len + 1;
+        fields[4 * e] = o_seq;
+        fields[4 * e + 1] = nb;
+        fields[4 * e + 2] = o_seq + nb;
+        fields[4 * e + 3] = rr.out_len;
+        at = o_seq + nb + rr.out_len + 3 + o.co_len + 1;
+    }
+    *text_len = (int64_t)all.size();
+    *stream_len = at - stream_base;
+    if (n_emitted) *n_emitted = (int32_t)emit.size();
+    if (bases_emitted) *bases_emitted = total - bases_so_far;
+    if (next_read) *next_read = (int32_t)next_j;
+    if ((int64_t)all.size() > text_cap || (!all.empty() && !text)) return BB_ERR_CAPACITY;
+    if (!all.empty()) std::memcpy(text, all.data(), all.size());
+    return BB_OK;
+}
+
+extern "C" int bb_fastq_format(const bb_plan_view *v,const bb_read_result *results, const uint8_t *seq, const uint8_t *qual,
                                int32_t first, int64_t bases_so_far, int64_t target_bases, int32_t n_threads, uint8_t *out,
                                int64_t out_cap, int64_t *out_len, int32_t *n_emitted, int64_t *bases_emitted,
                                int32_t *next_read) {

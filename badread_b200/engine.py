@@ -316,6 +316,73 @@ class Engine(object):
         self._check(rc, 'bb_bgzf_compress')
         return self._bgzf_buf[:n_out.value], int(n_used.value)
 
+    # ---- BAM output (badread_b200/bam.py)
+    def run_batch_results(self, batch):
+        """Uploads, runs and fetches a batch like sequence_batch, but leaves the bases and qualities on the device for
+        bam_build (bb_fetch_last_batch_results); returns (BatchResult without seq / qual, total_bases)."""
+        self.upload_batch(batch)
+        self.run_batch()
+        n = self._n
+        results = (ReadResult * n)()
+        total = ctypes.c_int64(0)
+        self._check(self._lib.bb_fetch_last_batch_results(self._ctx, results, ctypes.byref(total)), 'bb_fetch_last_batch_results')
+        return BatchResult(results, None, None, n), int(total.value)
+
+    def bam_build(self, recs, text):
+        """Appends BAM records of the last batch to this GPU's record stream (bb_bam_build): recs is an array of
+        planner.BAM_RECORD_DTYPE, text the pool their text_off index."""
+        recs = np.ascontiguousarray(recs)
+        text = np.ascontiguousarray(np.frombuffer(text, dtype=np.uint8) if isinstance(text, (bytes, bytearray)) else text)
+        self._check(self._lib.bb_bam_build(self._ctx, len(recs), _ptr(recs) if len(recs) else None,
+                                           _ptr(text) if text.size else None, text.size), 'bb_bam_build')
+
+    def _members_buf(self, need):
+        if self._bgzf_buf is None or self._bgzf_buf.size < need:
+            cap = max(need + need // 8, 1 << 20)
+            p = ctypes.c_void_p()
+            if self._lib.bb_host_alloc(ctypes.byref(p), cap) != 0:
+                raise EngineError(f'bb_host_alloc({cap}) failed')
+            self._pinned.append(p)
+            self._bgzf_buf = np.ctypeslib.as_array((ctypes.c_uint8 * cap).from_address(p.value))
+        return self._bgzf_buf
+
+    def bam_compress_device(self, final=False):
+        """BGZF members of the whole chunks of the record stream (all of it with `final`); the rest stays on the device.
+        Returns a uint8 array in page-locked memory that the next call reuses."""
+        n_out = ctypes.c_int64(0)
+        buf = self._bgzf_buf
+        rc = self._lib.bb_bam_compress_device(self._ctx, int(bool(final)), _ptr(buf) if buf is not None else None,
+                                              buf.size if buf is not None else 0, ctypes.byref(n_out))
+        if rc == _lib.BB_ERR_CAPACITY:
+            buf = self._members_buf(n_out.value)
+            rc = self._lib.bb_bam_compress_device(self._ctx, int(bool(final)), _ptr(buf), buf.size, ctypes.byref(n_out))
+        self._check(rc, 'bb_bam_compress_device')
+        return buf[:n_out.value] if n_out.value else np.zeros(0, np.uint8)
+
+    def bam_fetch_records(self, out, dst_off=None):
+        """Copies the records of the last bam_build into the uint8 array out (record i at dst_off[i], or back to back) and
+        takes them off the record stream; returns their size in bytes."""
+        n = ctypes.c_int64(0)
+        off = np.ascontiguousarray(dst_off, dtype=np.int64) if dst_off is not None else None
+        self._check(self._lib.bb_bam_fetch_records(self._ctx, _ptr(off) if off is not None and off.size else None,
+                                                   _ptr(out) if out.size else None, out.size, ctypes.byref(n)),
+                    'bb_bam_fetch_records')
+        return int(n.value)
+
+    def bam_compress(self, buf, stream_base, fields, final=False):
+        """BGZF members of host bytes of a record stream (bb_bam_compress): buf starts at byte stream_base of the stream,
+        fields is an (n, 2) int64 array of the (stream offset, length) of its seq and qual fields.  Returns (members, bytes
+        of buf consumed) like bgzf_compress."""
+        data = np.frombuffer(buf, dtype=np.uint8)
+        f = np.ascontiguousarray(fields, dtype=np.int64).reshape(-1, 2)
+        buf_out = self._members_buf(int(self._lib.bb_bgzf_bound(data.size)))
+        n_out, n_used = ctypes.c_int64(0), ctypes.c_int64(0)
+        rc = self._lib.bb_bam_compress(self._ctx, _ptr(data) if data.size else None, data.size, int(stream_base),
+                                       _ptr(f) if len(f) else None, len(f), int(bool(final)), _ptr(buf_out), buf_out.size,
+                                       ctypes.byref(n_out), ctypes.byref(n_used))
+        self._check(rc, 'bb_bam_compress')
+        return buf_out[:n_out.value], int(n_used.value)
+
     # ---- the one collective: SUM of emitted bases over the GPUs (stop condition, simulate.py:63)
     def comm_init_rank(self, unique_id, rank, world):
         """One process per GPU: joins the NCCL communicator identified by `unique_id` (128 bytes from

@@ -203,3 +203,50 @@ def fastq_format_sharded(planned, results, seq_bufs, qual_bufs, first, bases_so_
     if rc != 0:
         raise RuntimeError(f'bb_fastq_format_sharded failed ({rc})')
     return (out[:need.value] if out is not None else np.zeros(0, np.uint8)), n_emit.value, bases.value, nxt.value, out
+
+
+BAM_RECORD_DTYPE = np.dtype([('out_off', np.int64), ('text_off', np.int64), ('out_len', np.int32), ('name_len', np.int32),
+                             ('co_len', np.int32), ('reserved', np.int32)])
+assert BAM_RECORD_DTYPE.itemsize == ctypes.sizeof(_lib.BamRecord)
+
+
+class BamLayout(object):
+    """bb_bam_layout_sharded: where the BAM records of a batch's emitted reads go.  Per emitted record e: shard[e] and
+    index[e] (the read's shard and position in that shard's results), stream_off[e] (its offset in the record stream),
+    recs[e] (a bb_bam_record, text_off into text) and fields[2 e], fields[2 e + 1] (stream offset, length) of its seq and
+    qual field.  stream_len: bytes of the records."""
+
+    def __init__(self, shard, index, stream_off, recs, fields, text, stream_len, n_emitted, bases, next_read):
+        self.shard, self.index, self.stream_off, self.recs, self.fields, self.text = shard, index, stream_off, recs, fields, text
+        self.stream_len, self.n_emitted, self.bases, self.next_read = stream_len, n_emitted, bases, next_read
+
+
+def bam_layout_sharded(planned, results, first, bases_so_far, target_bases, stream_base=0):
+    """The BAM records (bb_bam_build) of the reads fastq_format_sharded would emit for the same arguments."""
+    L = _lib.lib()
+    G = len(planned)
+    n = sum(len(p) for p in planned)
+    views = (ctypes.c_void_p * G)(*[ctypes.addressof(p.view) for p in planned])
+    res = (ctypes.c_void_p * G)(*[ctypes.addressof(r) for r in results])
+    shard, index = np.empty(max(n, 1), np.int32), np.empty(max(n, 1), np.int32)
+    stream_off = np.empty(max(n, 1), np.int64)
+    recs = np.empty(max(n, 1), BAM_RECORD_DTYPE)
+    fields = np.empty((max(n, 1) * 2, 2), np.int64)
+    text_len, stream_len = ctypes.c_int64(0), ctypes.c_int64(0)
+    n_emit, bases, nxt = ctypes.c_int32(0), ctypes.c_int64(0), ctypes.c_int32(0)
+    text = np.empty(n * 192 + 1, np.uint8)
+
+    def call(t):
+        return L.bb_bam_layout_sharded(G, views, res, int(first), int(bases_so_far), int(target_bases), int(stream_base),
+                                       shard.ctypes.data, index.ctypes.data, stream_off.ctypes.data, recs.ctypes.data,
+                                       fields.ctypes.data, t.ctypes.data, t.size, ctypes.byref(text_len),
+                                       ctypes.byref(stream_len), ctypes.byref(n_emit), ctypes.byref(bases), ctypes.byref(nxt))
+    rc = call(text)
+    if rc == _lib.BB_ERR_CAPACITY:
+        text = np.empty(text_len.value + 1, np.uint8)
+        rc = call(text)
+    if rc != 0:
+        raise RuntimeError(f'bb_bam_layout_sharded failed ({rc})')
+    e = n_emit.value
+    return BamLayout(shard[:e], index[:e], stream_off[:e], recs[:e], fields[:2 * e], text[:text_len.value], stream_len.value,
+                     e, bases.value, nxt.value)

@@ -481,7 +481,8 @@ def run_batches(args, ref, frag_lengths, identities, error_model, qscore_model, 
     indices is dealt out over the GPUs (GPU g takes indices = g mod G), planned by the native planner, sequenced on
     the GPUs side by side (one host thread each) and written in index order until the total reaches the target, so
     the FASTQ is independent of the batch size and of the number of GPUs.  With --gzip the GPUs compress the FASTQ to
-    BGZF (badread_b200/bgzf.py) before it is written."""
+    BGZF (badread_b200/bgzf.py) before it is written; with --bam they build and compress unaligned BAM records of the
+    same reads instead (badread_b200/bam.py)."""
     from .planner import NativePlanner, fastq_format_sharded
     from ._lib import ReadResult
     import os
@@ -510,7 +511,11 @@ def run_batches(args, ref, frag_lengths, identities, error_model, qscore_model, 
     out_buf = None
     empty = np.zeros(1, dtype=np.uint8)
     writer = None
-    if getattr(args, 'gzip', False):
+    bam = getattr(args, 'bam', False)
+    if bam:   # records built and compressed on the GPUs: the bases and qualities stay on the device
+        from .bam import BAMWriter
+        writer = BAMWriter(engines, _binary(stdout))
+    elif getattr(args, 'gzip', False):
         from .bgzf import BGZFWriter
         writer = BGZFWriter(engines, _binary(stdout))
     print_progress(count, total_size, target_size, output)
@@ -524,7 +529,12 @@ def run_batches(args, ref, frag_lengths, identities, error_model, qscore_model, 
                 try:
                     n_g = len(range(g, n_batch, n_gpus))
                     planned[g] = planners[g].plan(next_index + g, n_g, stride=n_gpus)
-                    results[g] = engines[g].sequence_batch(planned[g])[0] if n_g else None
+                    if not n_g:
+                        results[g] = None
+                    elif bam:
+                        results[g] = engines[g].run_batch_results(planned[g])[0]
+                    else:
+                        results[g] = engines[g].sequence_batch(planned[g])[0]
                 except BaseException as e:   # re-raised on the main thread (a worker thread would swallow it)
                     errors[g] = e
 
@@ -540,14 +550,17 @@ def run_batches(args, ref, frag_lengths, identities, error_model, qscore_model, 
                 if e is not None:
                     raise e
             recs = [r.records if r is not None else (ReadResult * 1)() for r in results]
-            seqs = [r.seq if r is not None else empty for r in results]
-            quals = [r.qual if r is not None else empty for r in results]
-            buf, n_emit, bases, _, out_buf = fastq_format_sharded(planned, recs, seqs, quals, 0, total_size, target_size,
-                                                                  out=out_buf)
-            if writer is None:
-                _write_fastq(stdout, buf)
+            if bam:
+                n_emit, bases = writer.write_batch(planned, recs, total_size, target_size)
             else:
-                writer.write(buf)
+                seqs = [r.seq if r is not None else empty for r in results]
+                quals = [r.qual if r is not None else empty for r in results]
+                buf, n_emit, bases, _, out_buf = fastq_format_sharded(planned, recs, seqs, quals, 0, total_size, target_size,
+                                                                      out=out_buf)
+                if writer is None:
+                    _write_fastq(stdout, buf)
+                else:
+                    writer.write(buf)
             if use_nccl:
                 # every GPU learns the batch's total from one all-reduce: more than was written means the target was
                 # reached inside this batch (the FASTQ stops after the read that reaches it, simulate.py:63)

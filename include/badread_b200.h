@@ -219,6 +219,50 @@ BB_API int64_t bb_bgzf_bound(int64_t n);
 BB_API int bb_bgzf_compress(bb_ctx *ctx, const uint8_t *in, int64_t n, int line_mod4, int final, uint8_t *out, int64_t out_cap,
                             int64_t *n_out, int64_t *n_consumed);
 
+/* ---- BAM output ------------------------------------------------------------------------------------- */
+/* Unaligned BAM records (SAM specification v1.6 §4.2) of the last batch, built on the device from the workers' output
+ * buffers, so that with one GPU the bases and qualities never cross PCIe before they are compressed.  A record is
+ * refID -1, pos -1, bin 4680, MAPQ 0, FLAG 4, no CIGAR, next_refID -1, next_pos -1, tlen 0, the read name, seq as 4-bit
+ * =ACMGRSVTWYHKDBN codes (either case; any other byte is N), qual = the FASTQ quality character - 33, and one CO:Z tag.
+ * The records form a record stream (the BAM file after its header) that the context keeps on the device: the records of
+ * each bb_bam_build are appended to it.
+ *
+ *  bb_fetch_last_batch_results: bb_fetch_last_batch without the bases and qualities, which stay on the device for
+ *  bb_bam_build.  *out_total = bytes of output the batch holds.
+ *
+ *  bb_bam_build: appends one record per recs[i] (in order) to the record stream.  recs[i].out_off / out_len are a read's
+ *  out_off / out_len in the last fetched batch's results; its name (name_len bytes, at most 254) and its CO text (co_len
+ *  bytes) lie back to back at text[recs[i].text_off ..].  Runs on the context's own stream and scratch; the workers'
+ *  buffers are only read.  BB_ERR_STATE if no batch was fetched; BB_ERR_ARG for a record outside the batch or the text.
+ *
+ *  bb_bam_compress_device: compresses the record stream as BGZF members of BB_BGZF_CHUNK bytes at fixed offsets of the
+ *  stream, a deflate block starting at every seq or qual field with at least 1024 bytes in the member.  Without `final`
+ *  only whole chunks are compressed and the rest (< BB_BGZF_CHUNK bytes) stays on the device for the next call.  out_cap
+ *  must be at least bb_bgzf_bound(bytes to be compressed), else BB_ERR_CAPACITY with *n_out = that bound.
+ *
+ *  bb_bam_fetch_records: copies the records of the last bb_bam_build to the host and takes them off the record stream
+ *  (for a record stream merged from several GPUs).  Record i goes to out[dst_off[i] ..], or back to back if dst_off is
+ *  NULL; out_cap bounds every write.  *n_bytes = the bytes of the records.  BB_ERR_STATE if the stream was compressed
+ *  since that build.
+ *
+ *  bb_bam_compress: compresses the host bytes in[0..n) of a record stream, in[0] being byte stream_base of the stream,
+ *  the way bb_bam_compress_device does: fields[2 * n_fields] are the (stream offset, length) pairs of the seq and qual
+ *  fields in stream order (fields outside in[] are ignored).  Consumed bytes, capacity and `final` as bb_bgzf_compress. */
+typedef struct bb_bam_record {
+    int64_t out_off;   /* the read's out_off in the batch results */
+    int64_t text_off;  /* its name, then its CO text, in the text pool */
+    int32_t out_len;   /* l_seq */
+    int32_t name_len;  /* bytes of the name, without a NUL */
+    int32_t co_len;    /* bytes of the CO text, without a NUL */
+    int32_t reserved;
+} bb_bam_record;
+BB_API int bb_fetch_last_batch_results(bb_ctx *ctx, bb_read_result *results, int64_t *out_total);
+BB_API int bb_bam_build(bb_ctx *ctx, int32_t n_records, const bb_bam_record *recs, const uint8_t *text, int64_t text_len);
+BB_API int bb_bam_compress_device(bb_ctx *ctx, int final, uint8_t *out, int64_t out_cap, int64_t *n_out);
+BB_API int bb_bam_fetch_records(bb_ctx *ctx, const int64_t *dst_off, uint8_t *out, int64_t out_cap, int64_t *n_bytes);
+BB_API int bb_bam_compress(bb_ctx *ctx, const uint8_t *in, int64_t n, int64_t stream_base, const int64_t *fields,
+                           int64_t n_fields, int final, uint8_t *out, int64_t out_cap, int64_t *n_out, int64_t *n_consumed);
+
 /* ---- BGZF input ------------------------------------------------------------------------------------- */
 /* Inflates the BGZF stream in[0..n) on `device` (any number of members, the end-of-file member included) into out: one warp
  * per member, all three deflate block types, every member's CRC-32 and ISIZE checked.  Like the model builders' calls it
@@ -324,6 +368,19 @@ BB_API int bb_fastq_format_sharded(int32_t n_shards, const bb_plan_view *const *
                             const uint8_t *const *seq, const uint8_t *const *qual, int32_t first, int64_t bases_so_far,
                             int64_t target_bases, int32_t n_threads, uint8_t *out, int64_t out_cap, int64_t *out_len,
                             int32_t *n_emitted, int64_t *bases_emitted, int32_t *next_read);
+/* The layout of the BAM records (bb_bam_build) of the same emitted set and cutoff as bb_fastq_format_sharded for the same
+ * arguments, the first record starting at byte stream_base of the record stream.  For emitted record e: shard[e] and
+ * index[e] (the read's shard and its position in that shard's results), stream_off[e], recs[e] (out_off and out_len from
+ * the results; text_off into text) and fields[4 e ..] = stream offset and length of its seq field, then of its qual field.
+ * shard, index, stream_off, recs and fields hold an entry for every read of the batch.  The name is the UUID of the FASTQ
+ * header and the CO text the rest of its header line ("{info} length=... error-free_length=... read_identity=...%"),
+ * formatted by the code that writes the FASTQ header.  *text_len = bytes of text needed (BB_ERR_CAPACITY if text_cap is
+ * smaller), *stream_len = bytes of the records. */
+BB_API int bb_bam_layout_sharded(int32_t n_shards, const bb_plan_view *const *views, const bb_read_result *const *results,
+                                 int32_t first, int64_t bases_so_far, int64_t target_bases, int64_t stream_base,
+                                 int32_t *shard, int32_t *index, int64_t *stream_off, bb_bam_record *recs, int64_t *fields,
+                                 uint8_t *text, int64_t text_cap, int64_t *text_len, int64_t *stream_len,
+                                 int32_t *n_emitted, int64_t *bases_emitted, int32_t *next_read);
 
 /* ---- Model builders: the counting passes of `badread error_model` (badread/error_model.py:31-83) and `badread
  * qscore_model` (badread/qscore_model.py:78-161) on the GPU.  The caller has parsed the inputs and chosen the alignments
