@@ -104,6 +104,10 @@ def lib():
         'bb_last_error': (c.c_char_p, [vp]),
         'bb_version': (c.c_char_p, []),
         'bb_upload_reference': (c.c_int, [vp, vp, i64]),
+        'bb_fasta_parse': (c.c_int, [vp, vp, i64, c.c_int, P(i32), P(i64), P(i64)]),
+        'bb_fasta_headers': (c.c_int, [vp, vp, i64, vp, vp, i32]),
+        'bb_fasta_reference': (c.c_int, [vp, i32, vp, vp]),
+        'bb_download_reference': (c.c_int, [vp, i64, i64, vp]),
         'bb_upload_error_model': (c.c_int, [vp, c.c_int, c.c_int, vp, i64, i32, vp, vp, vp, vp, vp, i64]),
         'bb_upload_error_model_kmers': (c.c_int, [vp, c.c_int, i32, vp, vp, vp, vp, vp, vp, i64]),
         'bb_upload_qscore_model': (c.c_int, [vp, c.c_int, i32, vp, vp, vp, vp]),
@@ -178,4 +182,5 @@ EXPORTED_SYMBOLS = ['bb_create', 'bb_destroy', 'bb_last_error', 'bb_version', 'b
                     'bb_count_kmer_alternatives', 'bb_count_kmer_alternatives_wide', 'bb_count_cigar_qscores', 'bb_model_error',
                     'bb_bgzf_bound', 'bb_bgzf_compress', 'bb_bgzf_decompress', 'bb_aln_parse', 'bb_aln_view_get', 'bb_aln_free',
                     'bb_fetch_last_batch_results', 'bb_bam_build', 'bb_bam_compress_device', 'bb_bam_fetch_records',
-                    'bb_bam_compress', 'bb_bam_layout_sharded']
+                    'bb_bam_compress', 'bb_bam_layout_sharded', 'bb_fasta_parse', 'bb_fasta_headers', 'bb_fasta_reference',
+                    'bb_download_reference']

@@ -195,6 +195,10 @@ struct bb_ctx {
 
     // reference + models, shared by the workers
     DevBuf ref; int64_t ref_len = 0;
+    // a FASTA parsed by bb_fasta_parse (fa_n_kept >= 0): its kept bytes, header texts and each header's kept offset,
+    // until bb_fasta_reference forms the reference from them
+    DevBuf fa_kept; int64_t fa_n_kept = -1;
+    std::string fa_text; std::vector<int64_t> fa_text_off, fa_kept_off;
     bool have_em = false, have_qm = false;
     BBErrorModelDev em{}; DevBuf em_k2r, em_rowoff, em_cum, em_flags, em_slots, em_pool, em_rowinfo;
     BBEmHashDev em_hash{}; DevBuf em_hentries;  // k-mer index as a hash table (bb_upload_error_model_kmers)
@@ -406,6 +410,144 @@ extern "C" int bb_upload_reference(bb_ctx *ctx, const uint8_t *bases, int64_t n_
     if (rc) return rc;
     BB_CUDA(ctx, cudaStreamSynchronize(st));
     ctx->ref_len = n_bases;
+    return BB_OK;
+}
+
+extern "C" int bb_download_reference(bb_ctx *ctx, int64_t offset, int64_t n, uint8_t *out) {
+    if (!ctx || offset < 0 || n < 0 || (n && !out)) return set_err(ctx, BB_ERR_ARG, "bb_download_reference: bad arguments");
+    if (offset + n > ctx->ref_len) return set_err(ctx, BB_ERR_ARG, "bb_download_reference: range beyond the reference");
+    BB_CUDA(ctx, cudaSetDevice(ctx->device));
+    if (n) BB_CUDA(ctx, cudaMemcpy(out, ctx->ref.as<uint8_t>() + offset, (size_t)n, cudaMemcpyDeviceToHost));
+    return BB_OK;
+}
+
+// ---- the reference from a FASTA file parsed on the device (bb_fasta.cuh)
+// Exactly `bytes` (at least 1) in buf: the loader's buffers are the size of the reference, so no slack.
+static cudaError_t alloc_exact(DevBuf &buf, size_t bytes) {
+    buf.release();
+    bytes = std::max<size_t>(bytes, 1);
+    cudaError_t e = cudaMalloc(&buf.p, bytes);
+    if (e == cudaSuccess) buf.cap = bytes;
+    return e;
+}
+
+static void fasta_reset(bb_ctx *ctx) {
+    ctx->fa_kept.release();
+    ctx->fa_n_kept = -1;
+    ctx->fa_text.clear();
+    ctx->fa_text_off.clear();
+    ctx->fa_kept_off.clear();
+}
+
+extern "C" int bb_fasta_parse(bb_ctx *ctx, const uint8_t *data, int64_t n, int is_bgzf, int32_t *n_headers, int64_t *text_bytes,
+                              int64_t *n_kept) {
+    if (!ctx || n < 0 || (n && !data) || !n_headers || !text_bytes || !n_kept)
+        return set_err(ctx, BB_ERR_ARG, "bb_fasta_parse: bad arguments");
+    BB_CUDA(ctx, cudaSetDevice(ctx->device));
+    for (const auto &w : ctx->workers) BB_CUDA(ctx, cudaStreamSynchronize(w->stream));
+    fasta_reset(ctx);
+    ctx->ref.release();   // (replaced by bb_fasta_reference; freed first, so that the parse has its memory)
+    ctx->ref_len = 0;
+    const cudaStream_t st = ctx->w0().stream;
+    DevBuf text, scratch, hdr, idx, htext;
+    int64_t len = n;
+    if (is_bgzf) {
+        uint8_t *p = nullptr;
+        char msg[256];
+        if (const int rc = bbl_bgzf_inflate_device(st, data, n, &p, &len, msg, sizeof(msg))) return set_err(ctx, rc, msg);
+        text.p = p;
+        text.cap = (size_t)std::max<int64_t>(len, 16);
+    } else {
+        BB_CUDA(ctx, alloc_exact(text, (size_t)n));
+        if (n) BB_CUDA(ctx, cudaMemcpyAsync(text.p, data, (size_t)n, cudaMemcpyHostToDevice, st));
+    }
+    BB_CUDA(ctx, alloc_exact(scratch, bbl_fasta_scratch_bytes(len)));
+    bbl_fasta_scan(st, text.as<uint8_t>(), len, scratch.p);
+    int64_t totals[2] = {0, 0};
+    BB_CUDA(ctx, cudaMemcpyAsync(totals, bbl_fasta_totals(scratch.p, len), sizeof(totals), cudaMemcpyDeviceToHost, st));
+    BB_CUDA(ctx, cudaStreamSynchronize(st));
+    const int64_t kept = totals[0], nh = totals[1];
+    if (nh > INT32_MAX) return set_err(ctx, BB_ERR_ARG, "bb_fasta_parse: more than 2^31 - 1 header lines");
+    BB_CUDA(ctx, alloc_exact(ctx->fa_kept, (size_t)kept));
+    BB_CUDA(ctx, alloc_exact(hdr, 3 * sizeof(int64_t) * (size_t)nh));
+    int64_t *d_start = hdr.as<int64_t>(), *d_end = d_start + nh, *d_kept = d_end + nh;
+    bbl_fasta_emit(st, text.as<uint8_t>(), len, scratch.p, ctx->fa_kept.as<uint8_t>(), d_start, d_end, d_kept);
+    BB_CUDA(ctx, cudaGetLastError());
+    std::vector<int64_t> h((size_t)(3 * nh));
+    if (nh) BB_CUDA(ctx, cudaMemcpyAsync(h.data(), hdr.p, h.size() * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    BB_CUDA(ctx, cudaStreamSynchronize(st));
+    // the header texts (after the '>', up to the newline) gathered into one buffer
+    std::vector<int64_t> lo_off((size_t)(2 * nh + 1));
+    lo_off[(size_t)nh] = 0;
+    for (int64_t k = 0; k < nh; k++) {
+        lo_off[(size_t)k] = h[(size_t)k] + 1;
+        lo_off[(size_t)(nh + k + 1)] = lo_off[(size_t)(nh + k)] + (h[(size_t)(nh + k)] - h[(size_t)k] - 1);
+    }
+    const int64_t tlen = lo_off[(size_t)(2 * nh)];
+    ctx->fa_text.resize((size_t)tlen);
+    if (tlen) {
+        if (const int rc = upload(ctx, st, idx, lo_off.data(), lo_off.size())) return rc;
+        BB_CUDA(ctx, alloc_exact(htext, (size_t)tlen));
+        bbl_fasta_gather(st, text.as<uint8_t>(), idx.as<int64_t>(), idx.as<int64_t>() + nh, (int32_t)nh, tlen, htext.as<uint8_t>());
+        BB_CUDA(ctx, cudaGetLastError());
+        BB_CUDA(ctx, cudaMemcpyAsync(&ctx->fa_text[0], htext.p, (size_t)tlen, cudaMemcpyDeviceToHost, st));
+        BB_CUDA(ctx, cudaStreamSynchronize(st));
+    }
+    ctx->fa_text_off.assign(lo_off.begin() + nh, lo_off.end());
+    ctx->fa_kept_off.assign(h.begin() + 2 * nh, h.end());
+    ctx->fa_n_kept = kept;
+    *n_headers = (int32_t)nh;
+    *text_bytes = tlen;
+    *n_kept = kept;
+    return BB_OK;
+}
+
+extern "C" int bb_fasta_headers(bb_ctx *ctx, char *text, int64_t text_cap, int64_t *text_off, int64_t *kept_off, int32_t n_cap) {
+    if (!ctx || text_cap < 0 || n_cap < 0) return set_err(ctx, BB_ERR_ARG, "bb_fasta_headers: bad arguments");
+    if (ctx->fa_n_kept < 0) return set_err(ctx, BB_ERR_STATE, "bb_fasta_headers: no FASTA parsed (bb_fasta_parse)");
+    const size_t nh = ctx->fa_kept_off.size();
+    if ((size_t)n_cap < nh || (size_t)text_cap < ctx->fa_text.size())
+        return set_err(ctx, BB_ERR_CAPACITY, "bb_fasta_headers: " + std::to_string(nh) + " headers of " +
+                                                 std::to_string(ctx->fa_text.size()) + " bytes, capacity " + std::to_string(n_cap) +
+                                                 " of " + std::to_string(text_cap));
+    if (!text_off || !kept_off || (!ctx->fa_text.empty() && !text)) return set_err(ctx, BB_ERR_ARG, "bb_fasta_headers: bad arguments");
+    if (!ctx->fa_text.empty()) std::memcpy(text, ctx->fa_text.data(), ctx->fa_text.size());
+    std::copy(ctx->fa_text_off.begin(), ctx->fa_text_off.end(), text_off);
+    std::copy(ctx->fa_kept_off.begin(), ctx->fa_kept_off.end(), kept_off);
+    kept_off[nh] = ctx->fa_n_kept;
+    return BB_OK;
+}
+
+extern "C" int bb_fasta_reference(bb_ctx *ctx, int32_t n_contigs, const int64_t *lo, const int64_t *hi) {
+    if (!ctx || n_contigs < 0 || (n_contigs && (!lo || !hi))) return set_err(ctx, BB_ERR_ARG, "bb_fasta_reference: bad arguments");
+    if (ctx->fa_n_kept < 0) return set_err(ctx, BB_ERR_STATE, "bb_fasta_reference: no FASTA parsed (bb_fasta_parse)");
+    std::vector<int64_t> lo_off((size_t)(2 * n_contigs + 1));
+    bool in_place = true;   // the contigs are the kept bytes as they lie
+    for (int32_t c = 0; c < n_contigs; c++) {
+        if (lo[c] < 0 || lo[c] > hi[c] || hi[c] > ctx->fa_n_kept) return set_err(ctx, BB_ERR_ARG, "bb_fasta_reference: contig out of range");
+        lo_off[(size_t)c] = lo[c];
+        lo_off[(size_t)(n_contigs + c + 1)] = lo_off[(size_t)(n_contigs + c)] + (hi[c] - lo[c]);
+        in_place = in_place && lo[c] == (c ? hi[c - 1] : 0);
+    }
+    const int64_t total = lo_off[(size_t)(2 * n_contigs)];
+    in_place = in_place && total == ctx->fa_n_kept;
+    BB_CUDA(ctx, cudaSetDevice(ctx->device));
+    const cudaStream_t st = ctx->w0().stream;
+    if (in_place) {
+        ctx->ref.release();
+        std::swap(ctx->ref.p, ctx->fa_kept.p);
+        std::swap(ctx->ref.cap, ctx->fa_kept.cap);
+    } else {
+        DevBuf idx;
+        BB_CUDA(ctx, alloc_exact(ctx->ref, (size_t)total));
+        if (const int rc = upload(ctx, st, idx, lo_off.data(), lo_off.size())) return rc;
+        bbl_fasta_gather(st, ctx->fa_kept.as<uint8_t>(), idx.as<int64_t>(), idx.as<int64_t>() + n_contigs, n_contigs, total,
+                         ctx->ref.as<uint8_t>());
+        BB_CUDA(ctx, cudaGetLastError());
+        BB_CUDA(ctx, cudaStreamSynchronize(st));
+    }
+    ctx->ref_len = total;
+    fasta_reset(ctx);
     return BB_OK;
 }
 

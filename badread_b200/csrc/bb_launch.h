@@ -54,3 +54,19 @@ int64_t bbl_bam_record_size(int32_t name_len, int32_t l_seq, int32_t co_len);
 void bbl_bam_records(cudaStream_t st, int n_records, const bb_bam_record *recs, const int64_t *pos, const uint8_t *text,
                      int n_src, const uint8_t *const *seq, const uint8_t *const *qual, const int64_t *src_base, uint8_t *out,
                      int64_t stream_base, int64_t *fields);
+// FASTA (bb_fasta.cuh) of text[0..n) in device memory.  bbl_fasta_scan runs passes 1 and 2 in `scratch`
+// (bbl_fasta_scratch_bytes(n) bytes); then bbl_fasta_totals(scratch, n)[0] = the bytes kept, [1] = the header lines.
+// bbl_fasta_emit writes the kept bytes to kept[] and each header line's start, end and kept offset.
+size_t bbl_fasta_scratch_bytes(int64_t n);
+void bbl_fasta_scan(cudaStream_t st, const uint8_t *text, int64_t n, void *scratch);
+const int64_t *bbl_fasta_totals(const void *scratch, int64_t n);
+void bbl_fasta_emit(cudaStream_t st, const uint8_t *text, int64_t n, const void *scratch, uint8_t *kept, int64_t *hdr_start,
+                    int64_t *hdr_end, int64_t *hdr_kept);
+// dst[dst_off[r] .. dst_off[r + 1]) = src[src_lo[r] ..] for r < n_ranges; total = dst_off[n_ranges] (device arrays)
+void bbl_fasta_gather(cudaStream_t st, const uint8_t *src, const int64_t *src_lo, const int64_t *dst_off, int32_t n_ranges,
+                      int64_t total, uint8_t *dst);
+// BGZF in host memory in[0..n) inflated on `st` into a new device allocation *out of *total bytes (cudaFree it): the
+// input goes through a device buffer of its own, released before the call returns.  BB_ERR_ARG with msg naming the member
+// (index and offset) for input that is not BGZF or a corrupt member, as bb_bgzf_decompress; BB_ERR_CUDA otherwise.
+int bbl_bgzf_inflate_device(cudaStream_t st, const uint8_t *in, int64_t n, uint8_t **out, int64_t *total, char *msg,
+                            size_t msg_len);

@@ -11,6 +11,8 @@
 #include "bb_inflate.cuh"
 
 void bbm_set_error(const char *msg);   // bb_tu_models.cu
+int bbl_bgzf_inflate_device(cudaStream_t st, const uint8_t *in, int64_t n, uint8_t **out, int64_t *total, char *msg,
+                            size_t msg_len);   // (bb_launch.h)
 
 namespace {
 
@@ -72,5 +74,44 @@ extern "C" int bb_bgzf_decompress(int device, const uint8_t *in, int64_t n, uint
         return BB_ERR_ARG;
     }
     BBI_TRY(cudaMemcpy(out, d_out.p, (size_t)total, cudaMemcpyDeviceToHost));
+    return BB_OK;
+}
+
+int bbl_bgzf_inflate_device(cudaStream_t st, const uint8_t *in, int64_t n, uint8_t **out, int64_t *total, char *msg,
+                            size_t msg_len) {
+    *out = nullptr;
+    *total = 0;
+    std::vector<InflMember> members;
+    if (!infl_walk(in, n, members, total, msg, msg_len)) return BB_ERR_ARG;
+    auto fail = [&](const char *what, cudaError_t e) {
+        std::snprintf(msg, msg_len, "%s: %s", what, cudaGetErrorString(e));
+        return BB_ERR_CUDA;
+    };
+    DevBuf d_in, d_members, d_status, d_out;
+    cudaError_t e;
+    if ((e = cudaMalloc(&d_out.p, (size_t)(*total ? *total : 16))) != cudaSuccess) return fail("cudaMalloc", e);
+    if (!members.empty()) {
+        const int64_t n_members = (int64_t)members.size();
+        if ((e = cudaMalloc(&d_in.p, (size_t)n)) != cudaSuccess ||
+            (e = cudaMalloc(&d_members.p, members.size() * sizeof(InflMember))) != cudaSuccess ||
+            (e = cudaMalloc(&d_status.p, members.size() * sizeof(int32_t))) != cudaSuccess)
+            return fail("cudaMalloc", e);
+        if ((e = cudaMemcpyAsync(d_in.p, in, (size_t)n, cudaMemcpyHostToDevice, st)) != cudaSuccess ||
+            (e = cudaMemcpyAsync(d_members.p, members.data(), members.size() * sizeof(InflMember), cudaMemcpyHostToDevice,
+                                 st)) != cudaSuccess)
+            return fail("cudaMemcpyAsync", e);
+        const int64_t grid = (n_members + INFL_WARPS - 1) / INFL_WARPS;
+        infl_k_members<<<(unsigned)grid, INFL_THREADS, 0, st>>>((const uint8_t *)d_in.p, (const InflMember *)d_members.p,
+                                                                 n_members, (uint8_t *)d_out.p, (int32_t *)d_status.p);
+        if ((e = cudaGetLastError()) != cudaSuccess) return fail("infl_k_members", e);
+        std::vector<int32_t> status(members.size());
+        if ((e = cudaMemcpyAsync(status.data(), d_status.p, members.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, st)) !=
+                cudaSuccess ||
+            (e = cudaStreamSynchronize(st)) != cudaSuccess)
+            return fail("infl_k_members", e);
+        if (infl_first_failure(members, status.data(), msg, msg_len)) return BB_ERR_ARG;
+    }
+    *out = (uint8_t *)d_out.p;
+    d_out.p = nullptr;
     return BB_OK;
 }

@@ -10,6 +10,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import BB_SEG_LITERAL, BB_SEG_REF_FWD, BB_SEG_REF_REV, ReadResult, Segment
+from .misc import fasta_contigs
 
 
 _RESULT_DTYPE = np.dtype([('out_off', np.int64), ('out_len', np.int32), ('frag_len', np.int32), ('matches', np.int32),
@@ -89,6 +90,62 @@ class FragmentBatch(object):
                 np.ascontiguousarray(lit), len(self.literals), np.asarray(self.target_identity, dtype=np.float64))
 
 
+def _is_bgzf(head):
+    """Whether a gzip member header carries the BC extra field of BGZF (SAM specification §4.1)."""
+    if len(head) < 18 or head[:3] != b'\x1f\x8b\x08' or not head[3] & 4:
+        return False
+    xlen = int.from_bytes(head[10:12], 'little')
+    f, end = 12, min(12 + xlen, len(head))
+    while f + 4 <= end:
+        if head[f:f + 2] == b'BC':
+            return True
+        f += 4 + int.from_bytes(head[f + 2:f + 4], 'little')
+    return False
+
+
+class FastaFile(object):
+    """The bytes of a FASTA file as Engine.load_fasta takes them, read once for all the engines: a plain or BGZF file as
+    it is, in page-locked memory (bb_host_alloc) so that it goes to the GPUs at the link's rate, with BGZF inflated on
+    the GPUs; a gzip file that is not BGZF is inflated here.  close() releases the memory."""
+
+    def __init__(self, filename):
+        self._lib = _lib.lib()
+        self._pinned = None
+        with open(filename, 'rb') as f:
+            head = f.read(1 << 16)
+        self.bgzf = _is_bgzf(head)
+        if head[:2] == b'\x1f\x8b' and not self.bgzf:
+            import gzip
+            with gzip.open(filename, 'rb') as f:
+                self.data = np.frombuffer(f.read(), dtype=np.uint8)
+            return
+        size = os.path.getsize(filename)
+        p = ctypes.c_void_p()
+        if self._lib.bb_host_alloc(ctypes.byref(p), max(size, 1)) != 0:
+            raise EngineError(f'bb_host_alloc({size}) failed')
+        self._pinned = p
+        self.data = np.ctypeslib.as_array((ctypes.c_uint8 * max(size, 1)).from_address(p.value))[:size]
+        view, got = memoryview(self.data), 0
+        with open(filename, 'rb', buffering=0) as f:
+            while got < size:
+                n = f.readinto(view[got:got + (1 << 30)])
+                if not n:
+                    raise EngineError(f'{filename}: file shrank while being read')
+                got += n
+
+    def close(self):
+        self.data = None
+        if self._pinned is not None:
+            self._lib.bb_host_free(self._pinned)
+            self._pinned = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 class BatchResult(object):
     def __init__(self, results, seq, qual, n):
         self.records = results
@@ -155,6 +212,45 @@ class Engine(object):
         arr = np.frombuffer(bases, dtype=np.uint8) if isinstance(bases, (bytes, bytearray)) else np.ascontiguousarray(bases, dtype=np.uint8)
         self._ref_keepalive = arr
         self._check(self._lib.bb_upload_reference(self._ctx, _ptr(arr), arr.size), 'bb_upload_reference')
+
+    def load_fasta(self, fasta):
+        """Makes the reference of this GPU a FASTA file parsed on the GPU (bb_fasta_parse / bb_fasta_headers /
+        bb_fasta_reference) in place of upload_reference: the contigs that misc.load_fasta_arrays would give, concatenated,
+        without the bases ever being on the host.  fasta: a FastaFile, or a file name.  Returns (names, lengths, depths,
+        circular, hairpin_left, hairpin_right), the last four dicts by name as misc.fasta_contigs gives them."""
+        own = not isinstance(fasta, FastaFile)
+        if own:
+            fasta = FastaFile(fasta)
+        try:
+            n_hdr, n_text, n_kept = ctypes.c_int32(0), ctypes.c_int64(0), ctypes.c_int64(0)
+            data = fasta.data
+            self._check(self._lib.bb_fasta_parse(self._ctx, _ptr(data) if data.size else None, data.size, int(fasta.bgzf),
+                                                 ctypes.byref(n_hdr), ctypes.byref(n_text), ctypes.byref(n_kept)),
+                        'bb_fasta_parse')
+        finally:
+            if own:
+                fasta.close()
+        nh = n_hdr.value
+        text = ctypes.create_string_buffer(max(n_text.value, 1))
+        text_off = np.zeros(nh + 1, dtype=np.int64)
+        kept_off = np.zeros(nh + 1, dtype=np.int64)
+        self._check(self._lib.bb_fasta_headers(self._ctx, text, n_text.value, _ptr(text_off), _ptr(kept_off), nh),
+                    'bb_fasta_headers')
+        raw = text.raw
+        headers = [(raw[text_off[k]:text_off[k + 1]].decode('latin-1'), (int(kept_off[k]), int(kept_off[k + 1])))
+                   for k in range(nh)]
+        names, ranges, depths, circular, hp_left, hp_right = fasta_contigs(headers)
+        lo = np.asarray([r[0] for r in ranges] or [0], dtype=np.int64)
+        hi = np.asarray([r[1] for r in ranges] or [0], dtype=np.int64)
+        self._check(self._lib.bb_fasta_reference(self._ctx, len(ranges), _ptr(lo), _ptr(hi)), 'bb_fasta_reference')
+        return names, [b - a for a, b in ranges], depths, circular, hp_left, hp_right
+
+    def download_reference(self, offset=0, n=None):
+        """Bytes [offset, offset + n) of this GPU's reference (all from offset when n is None; the length is known to the
+        caller, who loaded it) as a uint8 array."""
+        out = np.zeros(max(int(n), 1), dtype=np.uint8)
+        self._check(self._lib.bb_download_reference(self._ctx, int(offset), int(n), _ptr(out)), 'bb_download_reference')
+        return out[:int(n)]
 
     def set_error_model(self, error_model, index='auto'):
         """index: how the device finds a k-mer's row.  'auto': the dense kmer_to_row[4^k] when the model has one

@@ -85,13 +85,41 @@ def load_fasta(filename):
 
 
 _UPPER = None
+_DEPTH_RE = re.compile(r'depth=([\d.]+)')
+
+
+def fasta_contigs(headers):
+    """The header semantics of load_fasta (misc.py:122-153), shared by load_fasta_arrays and the GPU loader
+    (engine.Engine.load_fasta).  headers: [(text of a header line after its '>', body)] in file order, body being whatever
+    the caller finds the contig's bases by.  A header that is empty once stripped names no contig; the name is the first
+    token; `depth=`, `circular=true` and `hairpin_left/right=true` are read from the lower-cased header; a repeated name
+    keeps its first position and its last body, like the reference's dict.  Returns (names, [body per name], depths,
+    circular, hairpin_left, hairpin_right), the last four dicts by name."""
+    names, bodies, depths, circular, hp_left, hp_right = [], {}, {}, {}, {}, {}
+    for text, body in headers:
+        header = text.strip()
+        if not header:
+            continue
+        short = header.split()[0]
+        lowered = header.lower()
+        depth = 1.0
+        if 'depth=' in lowered:
+            try:
+                depth = float(_DEPTH_RE.search(lowered).group(1))
+            except (ValueError, AttributeError):
+                depth = 1.0
+        if short not in bodies:
+            names.append(short)
+        bodies[short] = body
+        depths[short], circular[short] = depth, 'circular=true' in lowered
+        hp_left[short], hp_right[short] = 'hairpin_left=true' in lowered, 'hairpin_right=true' in lowered
+    return names, [bodies[n] for n in names], depths, circular, hp_left, hp_right
 
 
 def load_fasta_arrays(filename):
     """load_fasta (misc.py:122-153) for large references: the whole file is parsed with numpy (no per-line Python, no
     3 Gb Python strings).  Returns (names, [uint8 array per contig, upper-cased], depths, circular, hairpin_left,
-    hairpin_right) with the reference's header semantics (`depth=`, `circular=true`, `hairpin_*=true`, name = first
-    token); a repeated name keeps its last sequence, like the reference's dict."""
+    hairpin_right) with the reference's header semantics (fasta_contigs)."""
     global _UPPER
     import numpy as np
     if _UPPER is None:
@@ -112,31 +140,14 @@ def load_fasta_arrays(filename):
     ends = np.concatenate([nl, [data.size]])[:starts.size]       # its newline (or the end of the file)
     is_hdr = data[starts] == ord('>')
     hdr_lines = np.flatnonzero(is_hdr)
-    names, seqs, depths, circular, hp_left, hp_right = [], {}, {}, {}, {}, {}
-    depth_re = re.compile(r'depth=([\d.]+)')
-    keep = (data != 10) & (data != 13) & (data != 32) & (data != 9)
-    for k, li in enumerate(hdr_lines):
-        header = raw[starts[li] + 1:ends[li]].decode('latin-1').strip()
-        if not header:
-            continue
-        short = header.split()[0]
-        lowered = header.lower()
-        depth = 1.0
-        if 'depth=' in lowered:
-            try:
-                depth = float(depth_re.search(lowered).group(1))
-            except (ValueError, AttributeError):
-                depth = 1.0
-        lo = ends[li] + 1
+    headers = []
+    for k, li in enumerate(hdr_lines):   # a contig's body: from the end of its header line to the next header line
         hi = starts[hdr_lines[k + 1]] if k + 1 < hdr_lines.size else data.size
-        body = data[lo:hi]
-        seq = _UPPER[body[keep[lo:hi]]] if hi > lo else np.zeros(0, dtype=np.uint8)
-        if short not in seqs:
-            names.append(short)
-        seqs[short] = seq
-        depths[short], circular[short] = depth, 'circular=true' in lowered
-        hp_left[short], hp_right[short] = 'hairpin_left=true' in lowered, 'hairpin_right=true' in lowered
-    return names, [seqs[n] for n in names], depths, circular, hp_left, hp_right
+        headers.append((raw[starts[li] + 1:ends[li]].decode('latin-1'), (ends[li] + 1, hi)))
+    names, bodies, depths, circular, hp_left, hp_right = fasta_contigs(headers)
+    keep = (data != 10) & (data != 13) & (data != 32) & (data != 9)
+    seqs = [_UPPER[data[lo:hi][keep[lo:hi]]] if hi > lo else np.zeros(0, dtype=np.uint8) for lo, hi in bodies]
+    return names, seqs, depths, circular, hp_left, hp_right
 
 
 RANDOM_SEQ_DICT = {0: 'A', 1: 'C', 2: 'G', 3: 'T'}

@@ -28,7 +28,7 @@ import uuid
 import numpy as np
 
 from . import settings
-from .engine import Engine, FragmentBatch, default_engine, next_read_index
+from .engine import Engine, FastaFile, FragmentBatch, default_engine, next_read_index
 from .error_model import ErrorModel
 from .fragment_lengths import FragmentLengths
 from .identities import Identities
@@ -73,6 +73,9 @@ class Reference(object):
         self.right_hairpin = [right_hairpin[n] for n in self.names]
         self.offsets = np.concatenate([[0], np.cumsum(self.lengths)]).astype(np.int64)
         self.concat = np.concatenate(arrays) if arrays else np.zeros(0, dtype=np.uint8)
+        self._report(output)
+
+    def _report(self, output):
         plural = '' if len(self.names) == 1 else 's'
         print(f'  {len(self.names):,} contig{plural}:', file=output)
         for i, name in enumerate(self.names):
@@ -84,6 +87,46 @@ class Reference(object):
     @property
     def size(self):
         return int(sum(self.lengths))
+
+
+class DeviceReference(Reference):
+    """The reference FASTA loaded by the engines themselves: each one reads the file's bytes from one page-locked copy,
+    parses them on its GPU and keeps the contigs there (Engine.load_fasta), so the bases never exist on the host.  The
+    host keeps what the planner reads: names, lengths, depths and flags.  concat is None."""
+
+    def __init__(self, filename, engines, output=sys.stderr):
+        print('', file=output)
+        print(f'Loading reference from {filename}', file=output)
+        fasta = FastaFile(filename)
+        try:
+            tables = [None] * len(engines)
+            errors = [None] * len(engines)
+
+            def load(g):
+                try:
+                    tables[g] = engines[g].load_fasta(fasta)
+                except BaseException as e:   # re-raised on the main thread
+                    errors[g] = e
+
+            threads = [threading.Thread(target=load, args=(g,)) for g in range(1, len(engines))]
+            for t in threads:
+                t.start()
+            load(0)
+            for t in threads:
+                t.join()
+        finally:
+            fasta.close()
+        for e in errors:
+            if e is not None:
+                raise e
+        self.names, self.lengths, depths, circular, left_hairpin, right_hairpin = tables[0]
+        self.depths = [depths[n] for n in self.names]
+        self.circular = [circular[n] for n in self.names]
+        self.left_hairpin = [left_hairpin[n] for n in self.names]
+        self.right_hairpin = [right_hairpin[n] for n in self.names]
+        self.offsets = np.concatenate([[0], np.cumsum(self.lengths)]).astype(np.int64)
+        self.concat = None
+        self._report(output)
 
 
 def adjust_depths(ref, frag_lengths, args, rng):
@@ -425,7 +468,18 @@ def simulate(args, output=sys.stderr, stdout=None):
     seed = args.seed if args.seed is not None else random.SystemRandom().getrandbits(63)
     setup_rng = random.Random(seed)
     setup_nrng = np.random.RandomState(seed & 0xffffffff)
-    ref = Reference(args.reference, output)
+    n_gpus = max(1, int(getattr(args, 'gpus', 1) or 1))
+    engines = [Engine(device=g, seed=seed) for g in range(n_gpus)]   # each GPU parses the reference itself
+    try:
+        _simulate(args, output, stdout, seed, setup_rng, setup_nrng, engines)
+    finally:
+        for eng in engines:
+            eng.close()
+
+
+def _simulate(args, output, stdout, seed, setup_rng, setup_nrng, engines):
+    """simulate() once its engines exist: the reference is loaded onto them, then the reads are simulated."""
+    ref = DeviceReference(args.reference, engines, output)
     frag_lengths = FragmentLengths(args.mean_frag_length, args.frag_length_stdev, output)
     adjust_depths(ref, frag_lengths, args, setup_nrng)
     identities = Identities(args.mean_identity, args.identity_stdev, args.max_identity, output)
@@ -443,11 +497,10 @@ def simulate(args, output=sys.stderr, stdout=None):
     print(f'Target read set size: {target_size:,} bp', file=output)
     print('', file=output)
 
-    n_gpus = max(1, int(getattr(args, 'gpus', 1) or 1))
     import os
     import time
     t_loop = time.perf_counter()
-    stats = run_batches(args, ref, frag_lengths, identities, error_model, qscore_model, seed, target_size, n_gpus, output,
+    stats = run_batches(args, ref, frag_lengths, identities, error_model, qscore_model, seed, target_size, engines, output,
                         stdout)
     print('\n', file=output)
     if os.environ.get('BADREAD_B200_TIMING') == '1':   # one machine-readable line for bench.py's cli_e2e leg
@@ -476,8 +529,9 @@ def _binary(stdout):
     return raw
 
 
-def run_batches(args, ref, frag_lengths, identities, error_model, qscore_model, seed, target_size, n_gpus, output, stdout):
-    """The driver loop of simulate.py:63-86 over batches of reads.  Reads are numbered 0, 1, 2, ...; a batch of B
+def run_batches(args, ref, frag_lengths, identities, error_model, qscore_model, seed, target_size, engines, output, stdout):
+    """The driver loop of simulate.py:63-86 over batches of reads on the engines (one per GPU, each holding the
+    reference; the caller closes them).  Reads are numbered 0, 1, 2, ...; a batch of B
     indices is dealt out over the GPUs (GPU g takes indices = g mod G), planned by the native planner, sequenced on
     the GPUs side by side (one host thread each) and written in index order until the total reaches the target, so
     the FASTQ is independent of the batch size and of the number of GPUs.  With --gzip the GPUs compress the FASTQ to
@@ -486,14 +540,12 @@ def run_batches(args, ref, frag_lengths, identities, error_model, qscore_model, 
     from .planner import NativePlanner, fastq_format_sharded
     from ._lib import ReadResult
     import os
-    engines, planners = [], []
+    n_gpus = len(engines)
+    planners = []
     threads_each = max(1, (os.cpu_count() or 1) // n_gpus)
-    for g in range(n_gpus):
-        eng = Engine(device=g, seed=seed)
-        eng.upload_reference(ref.concat)
+    for eng in engines:
         eng.set_error_model(error_model)
         eng.set_qscore_model(qscore_model)
-        engines.append(eng)
         planners.append(NativePlanner(args, ref, frag_lengths, identities, seed, n_threads=threads_each))
 
     use_nccl = False
@@ -575,7 +627,5 @@ def run_batches(args, ref, frag_lengths, identities, error_model, qscore_model, 
         return {'reads': count, 'bases': total_size, 'gpus': n_gpus, 'batches_s': time.perf_counter() - t_first,
                 'nccl_stop_condition': bool(use_nccl)}
     finally:
-        for eng in engines:
-            eng.close()
         for pl in planners:
             pl.close()

@@ -84,6 +84,26 @@ BB_API const char *bb_version(void);
 /* Reference contigs concatenated (upper-case ASCII, misc.load_fasta misc.py:122-153). */
 BB_API int bb_upload_reference(bb_ctx *ctx, const uint8_t *bases, int64_t n_bases);
 
+/* The reference from a FASTA file parsed on the device, in place of bb_upload_reference: the bases never exist on the host.
+ * bb_fasta_parse takes the file's bytes (page-locked memory copies fastest): the FASTA text itself, or with is_bgzf its
+ * BGZF stream, inflated on the device as bb_bgzf_decompress inflates it (a gzip file that is not BGZF is inflated by the
+ * caller).  It drops the context's reference, then parses with the semantics of misc.load_fasta_arrays: a line starting
+ * with '>' is a header line; every other byte except '\n', '\r', ' ' and '\t' is kept, 'a'-'z' upper-cased.  It reports
+ * the number of header lines, the bytes of their texts and the bytes kept; BB_ERR_ARG names a corrupt BGZF member (index
+ * and offset) like bb_bgzf_decompress.  Device memory peaks at the input plus the text plus the kept bytes.
+ * bb_fasta_headers then copies the header table: text[text_off[k] .. text_off[k + 1]) the text of header line k after
+ * its '>' (without the newline, otherwise as in the file), kept_off[k] the bytes kept before it and kept_off[n] all of
+ * them, so contig k's bases are kept bytes [kept_off[k], kept_off[k + 1]).  BB_ERR_CAPACITY if n_cap or text_cap is
+ * smaller than what bb_fasta_parse reported.
+ * bb_fasta_reference makes the reference the concatenation of kept bytes [lo[c], hi[c]) for the n_contigs contigs (in
+ * place when they are all the kept bytes in order), as bb_upload_reference would, and releases the parse. */
+BB_API int bb_fasta_parse(bb_ctx *ctx, const uint8_t *data, int64_t n, int is_bgzf, int32_t *n_headers, int64_t *text_bytes,
+                          int64_t *n_kept);
+BB_API int bb_fasta_headers(bb_ctx *ctx, char *text, int64_t text_cap, int64_t *text_off, int64_t *kept_off, int32_t n_cap);
+BB_API int bb_fasta_reference(bb_ctx *ctx, int32_t n_contigs, const int64_t *lo, const int64_t *hi);
+/* Copies bytes [offset, offset + n) of the context's reference to out (for checking what a load left on the device). */
+BB_API int bb_download_reference(bb_ctx *ctx, int64_t offset, int64_t n, uint8_t *out);
+
 /* Error model tables (flat form of ErrorModel.alternatives / .probabilities, error_model.py:86-133):
  *  type 0 = 'random' (k = 1, no tables), 1 = 'model'.
  *  kmer_to_row[4^k]: row of each ACGT k-mer or -1; row_off[n_rows+1] entry ranges; per entry: cum (the
