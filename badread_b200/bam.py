@@ -12,12 +12,12 @@ several GPUs each builds the records of its own reads; they are copied back, mer
 chunks dealt out over the GPUs in contiguous runs, as BGZFWriter does for FASTQ.
 """
 import struct
-import threading
 
 import numpy as np
 
 from ._lib import BB_BGZF_CHUNK as BGZF_CHUNK
-from .bgzf import EOF_MEMBER
+from .bgzf import EOF_MEMBER, chunk_runs
+from .engine import run_each
 from .planner import bam_layout_sharded
 from .version import __version__
 
@@ -27,29 +27,6 @@ def header_bytes():
     line), no reference sequences."""
     text = (f'@HD\tVN:1.6\tSO:unknown\n@PG\tID:badread\tPN:badread\tVN:{__version__}\n').encode()
     return b'BAM\x01' + struct.pack('<i', len(text)) + text + struct.pack('<i', 0)
-
-
-def _run_each(n, work):
-    """work(k) for k < n, side by side on host threads; the first exception is raised on the caller's thread."""
-    errors = [None] * n
-
-    def run(k):
-        try:
-            work(k)
-        except BaseException as e:
-            errors[k] = e
-
-    if n == 1:
-        run(0)
-    else:
-        threads = [threading.Thread(target=run, args=(k,)) for k in range(n)]
-        for t in threads:
-            t.start()
-        for t in threads:
-            t.join()
-    for e in errors:
-        if e is not None:
-            raise e
 
 
 class BAMWriter(object):
@@ -83,7 +60,7 @@ class BAMWriter(object):
                     self.engines[g].bam_build(lay.recs[mine], lay.text)
                     self.engines[g].bam_fetch_records(merged, lay.stream_off[mine] - base)
 
-            _run_each(len(self.engines), build)
+            run_each(len(self.engines), build)
             self._write_host(merged, lay.fields)
         self.stream_len += lay.stream_len
         return lay.n_emitted, lay.bases
@@ -94,16 +71,15 @@ class BAMWriter(object):
         data = np.concatenate([np.frombuffer(self.tail, np.uint8), records]) if self.tail else records
         fields = np.concatenate([self.tail_fields, fields]) if len(self.tail_fields) else fields
         n_chunks = len(data) // BGZF_CHUNK
-        n_parts = max(1, min(len(self.engines), n_chunks))
-        per = -(-n_chunks // n_parts) * BGZF_CHUNK
-        bounds = [min(k * per, n_chunks * BGZF_CHUNK) for k in range(n_parts + 1)]
-        parts = [None] * n_parts
+        runs = chunk_runs(n_chunks, len(self.engines))
+        parts = [None] * len(runs)
 
         def work(k):
-            if bounds[k + 1] > bounds[k]:
-                parts[k] = bytes(self.engines[k].bam_compress(data[bounds[k]:bounds[k + 1]], base + bounds[k], fields)[0])
+            a, b = runs[k]
+            if b > a:
+                parts[k] = bytes(self.engines[k].bam_compress(data[a:b], base + a, fields)[0])
 
-        _run_each(n_parts, work)
+        run_each(len(runs), work)
         for p in parts:
             if p:
                 self.out.write(p)

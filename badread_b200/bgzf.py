@@ -10,12 +10,12 @@ Input (`decompress`): a whole BGZF file, BAM for the model builders, inflated on
 (csrc/bb_inflate.cuh).
 """
 import ctypes
-import threading
 
 import numpy as np
 
 from . import _lib
 from ._lib import BB_BGZF_CHUNK as BGZF_CHUNK
+from .engine import run_each
 
 # the empty member that ends a BGZF file (SAM specification §4.1.2)
 EOF_MEMBER = bytes.fromhex('1f8b08040000000000ff0600424302001b0003000000000000000000')
@@ -38,6 +38,14 @@ def decompress(data, device=0):
     if rc != _lib.BB_OK:
         raise RuntimeError('bgzf.decompress: ' + L.bb_model_error().decode(errors='replace'))
     return out
+
+
+def chunk_runs(n_chunks, n_engines):
+    """Chunks [0, n_chunks) dealt out over at most n_engines in contiguous runs of ceil(n_chunks / runs) chunks (the last
+    ones shorter, possibly empty): the byte bounds [(start, end)] of the runs, at least one."""
+    n_runs = max(1, min(n_engines, n_chunks))
+    per, end = -(-n_chunks // n_runs) * BGZF_CHUNK, n_chunks * BGZF_CHUNK
+    return [(min(k * per, end), min((k + 1) * per, end)) for k in range(n_runs)]
 
 
 def _newlines(buf):
@@ -71,25 +79,11 @@ class BGZFWriter(object):
         n_chunks = len(data) // BGZF_CHUNK
         parts = self._parts(data, n_chunks, mod4)
         results = [None] * len(parts)
-        errors = [None] * len(parts)
 
         def work(k):
-            try:
-                results[k] = self.engines[k].bgzf_compress(parts[k][0], parts[k][1], final=False)[0]
-            except BaseException as e:   # re-raised on the caller's thread
-                errors[k] = e
+            results[k] = self.engines[k].bgzf_compress(parts[k][0], parts[k][1], final=False)[0]
 
-        if len(parts) == 1:
-            work(0)
-        else:
-            threads = [threading.Thread(target=work, args=(k,)) for k in range(len(parts))]
-            for t in threads:
-                t.start()
-            for t in threads:
-                t.join()
-        for e in errors:
-            if e is not None:
-                raise e
+        run_each(len(parts), work)
         for members in results:
             self.out.write(members)
         self.tail = bytes(data[n_chunks * BGZF_CHUNK:])
@@ -97,18 +91,14 @@ class BGZFWriter(object):
 
     def _parts(self, data, n_chunks, mod4):
         """The whole chunks of data as [(slice, line index mod 4 at its start)], one contiguous run per engine."""
-        n_parts = max(1, min(len(self.engines), n_chunks))
-        per = -(-n_chunks // n_parts) * BGZF_CHUNK
-        bounds = [min(k * per, n_chunks * BGZF_CHUNK) for k in range(n_parts + 1)]
-        lines = [0] * n_parts
-        if n_parts > 1:   # newlines before each run, counted side by side
-            counters = [threading.Thread(target=lambda k=k: lines.__setitem__(k + 1, _newlines(data[bounds[k]:bounds[k + 1]])))
-                        for k in range(n_parts - 1)]
-            for t in counters:
-                t.start()
-            for t in counters:
-                t.join()
-        return [(data[bounds[k]:bounds[k + 1]], (mod4 + sum(lines[:k + 1])) & 3) for k in range(n_parts)]
+        runs = chunk_runs(n_chunks, len(self.engines))
+        lines = [0] * len(runs)
+
+        def count(k):   # the newlines of run k come before run k + 1; counted side by side
+            lines[k + 1] = _newlines(data[runs[k][0]:runs[k][1]])
+
+        run_each(len(runs) - 1, count)
+        return [(data[a:b], (mod4 + sum(lines[:k + 1])) & 3) for k, (a, b) in enumerate(runs)]
 
     def close(self):
         """Compresses the tail and ends the file with the end-of-file member."""

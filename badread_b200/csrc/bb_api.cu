@@ -183,6 +183,23 @@ struct Worker {
     }
 };
 
+// The BGZF compressor of a context (bb_bgzf_compress, bb_bam_compress*): a stream and scratch of its own, so that a call
+// leaves the workers alone.
+struct Bgzf {
+    cudaStream_t stream = nullptr;
+    int64_t *h = nullptr;   // pinned: line_pref[n_chunks] and offsets[n_chunks] of the last pass
+    DevBuf in, slots, lines, sizes, pref, off, out;
+    cudaError_t open() {   // the stream and the pinned words, made by the first call that needs them
+        cudaError_t e = stream ? cudaSuccess : cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking);
+        if (e == cudaSuccess && !h) e = cudaHostAlloc((void **)&h, 2 * sizeof(int64_t), cudaHostAllocPortable);
+        return e;
+    }
+    ~Bgzf() {
+        if (stream) cudaStreamDestroy(stream);
+        if (h) cudaFreeHost(h);
+    }
+};
+
 }  // namespace
 
 struct bb_ctx {
@@ -215,12 +232,9 @@ struct bb_ctx {
     void *nccl_comm = nullptr;   // ncclComm_t of this context's device (bb_comm_init_rank / bb_comm_init_all)
     DevBuf d_red;                // two int64: send, receive of bb_allreduce_bases
 
-    // BGZF compressor (bb_bgzf_compress): a stream and scratch of its own, so that a call leaves the workers alone
-    cudaStream_t bgzf_stream = nullptr;
-    int64_t *h_bgzf = nullptr;   // pinned: line_pref[n_chunks] and offsets[n_chunks] of the last pass
-    DevBuf bgzf_in, bgzf_slots, bgzf_lines, bgzf_sizes, bgzf_pref, bgzf_off, bgzf_out;
+    Bgzf bgzf;
 
-    // BAM output (bb_bam_*), on bgzf_stream.  The last fetched batch: its workers' blocks start at out_base[w] of the
+    // BAM output (bb_bam_*), on bgzf.stream.  The last fetched batch: its workers' blocks start at out_base[w] of the
     // concatenated output (out_base[n_split] = its size).
     bool fetched = false;
     std::vector<int64_t> out_base;
@@ -240,8 +254,6 @@ struct bb_ctx {
     Worker &w0() { return *workers[0]; }
     ~bb_ctx() {
         for (cudaEvent_t e : {ev_t0, ev_t1}) if (e) cudaEventDestroy(e);
-        if (bgzf_stream) cudaStreamDestroy(bgzf_stream);
-        if (h_bgzf) cudaFreeHost(h_bgzf);
         if (h_bam) cudaFreeHost(h_bam);
     }
 };
@@ -389,7 +401,7 @@ extern "C" int bb_destroy(bb_ctx *ctx) {
     if (!ctx) return BB_OK;
     cudaSetDevice(ctx->device);  // the frees below act on the current device
     for (const auto &w : ctx->workers) cudaStreamSynchronize(w->stream);
-    if (ctx->bgzf_stream) cudaStreamSynchronize(ctx->bgzf_stream);
+    if (ctx->bgzf.stream) cudaStreamSynchronize(ctx->bgzf.stream);
     if (ctx->nccl_comm && nccl_destroy) nccl_destroy(ctx->nccl_comm);
     delete ctx;
     return BB_OK;
@@ -1191,12 +1203,51 @@ extern "C" int64_t bb_bgzf_bound(int64_t n) {
 // against 34 ms with 2048.
 constexpr int64_t kBgzfPassChunks = 2048;
 
-// The compressor's stream and the pinned words its passes report through (created by the first call that needs them).
-static int ensure_bgzf_stream(bb_ctx *ctx) {
-    if (!ctx->bgzf_stream) {
-        BB_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->bgzf_stream, cudaStreamNonBlocking));
-        BB_CUDA(ctx, cudaHostAlloc((void **)&ctx->h_bgzf, 2 * sizeof(int64_t), cudaHostAllocPortable));
+// The start of every compress call (`who` names it in the messages): *use = the bytes it takes, all n with `final`,
+// else its whole chunks; the outputs zeroed (n_consumed may be null); out_cap checked against their bound, which
+// becomes *n_out when it is short; then the device and the compressor's stream, unless *use is 0.
+static int bgzf_begin(bb_ctx *ctx, const char *who, int64_t n, int final, const uint8_t *out, int64_t out_cap,
+                      int64_t *n_out, int64_t *n_consumed, int64_t *use) {
+    *use = final ? n : n / BB_BGZF_CHUNK * BB_BGZF_CHUNK;
+    *n_out = 0;
+    if (n_consumed) *n_consumed = 0;
+    if (bb_bgzf_bound(*use) > out_cap || (*use && !out)) {
+        *n_out = bb_bgzf_bound(*use);
+        return set_err(ctx, BB_ERR_CAPACITY, std::string(who) + ": out_cap is less than bb_bgzf_bound of the input");
     }
+    if (!*use) return BB_OK;
+    BB_CUDA(ctx, cudaSetDevice(ctx->device));
+    BB_CUDA(ctx, ctx->bgzf.open());
+    return BB_OK;
+}
+
+// Compresses `use` bytes in passes of at most kBgzfPassChunks chunks and copies the members to out (checked by
+// bgzf_begin).  enqueue(done, len, n_chunks) enqueues on the compressor's stream the kernels of the pass over input
+// bytes [done, done + len), which write the members to bgzf.out and their offsets to bgzf.off.
+template <typename Enqueue>
+static int bgzf_passes(bb_ctx *ctx, const char *who, int64_t use, uint8_t *out, int64_t *n_out, Enqueue &&enqueue) {
+    Bgzf &b = ctx->bgzf;
+    int64_t done = 0, written = 0;
+    while (done < use) {
+        const int64_t len = std::min(use - done, kBgzfPassChunks * BB_BGZF_CHUNK);
+        const int nc = (int)((len + BB_BGZF_CHUNK - 1) / BB_BGZF_CHUNK);
+        BB_CUDA(ctx, b.slots.ensure((size_t)nc * 65536));
+        BB_CUDA(ctx, b.sizes.ensure((size_t)nc * sizeof(int32_t)));
+        BB_CUDA(ctx, b.off.ensure((size_t)(nc + 1) * sizeof(int64_t)));
+        BB_CUDA(ctx, b.out.ensure((size_t)bb_bgzf_bound(len)));
+        if (const int rc = enqueue(done, len, nc)) return rc;
+        BB_CUDA(ctx, cudaGetLastError());
+        BB_CUDA(ctx, cudaMemcpyAsync(b.h + 1, b.off.as<int64_t>() + nc, sizeof(int64_t), cudaMemcpyDeviceToHost, b.stream));
+        BB_CUDA(ctx, cudaStreamSynchronize(b.stream));
+        const int64_t bytes = b.h[1];
+        if (bytes <= 0 || bytes > bb_bgzf_bound(len))
+            return set_err(ctx, BB_ERR_INTERNAL, std::string(who) + ": members of " + std::to_string(bytes) + " bytes");
+        BB_CUDA(ctx, cudaMemcpyAsync(out + written, b.out.p, (size_t)bytes, cudaMemcpyDeviceToHost, b.stream));
+        BB_CUDA(ctx, cudaStreamSynchronize(b.stream));
+        written += bytes;
+        done += len;
+    }
+    *n_out = written;
     return BB_OK;
 }
 
@@ -1204,48 +1255,25 @@ extern "C" int bb_bgzf_compress(bb_ctx *ctx, const uint8_t *in, int64_t n, int l
                                 int64_t out_cap, int64_t *n_out, int64_t *n_consumed) {
     if (!ctx || n < 0 || (n && !in) || line_mod4 < 0 || line_mod4 > 3 || out_cap < 0 || !n_out || !n_consumed)
         return set_err(ctx, BB_ERR_ARG, "bb_bgzf_compress: bad arguments");
-    const int64_t use = final ? n : n / BB_BGZF_CHUNK * BB_BGZF_CHUNK;
-    *n_out = 0;
-    *n_consumed = 0;
-    if (bb_bgzf_bound(use) > out_cap || (use && !out)) {
-        *n_out = bb_bgzf_bound(use);
-        return set_err(ctx, BB_ERR_CAPACITY, "bb_bgzf_compress: out_cap is less than bb_bgzf_bound of the input");
-    }
-    BB_CUDA(ctx, cudaSetDevice(ctx->device));
-    if (const int rc = ensure_bgzf_stream(ctx)) return rc;
-    const cudaStream_t st = ctx->bgzf_stream;
+    int64_t use;
+    if (const int rc = bgzf_begin(ctx, "bb_bgzf_compress", n, final, out, out_cap, n_out, n_consumed, &use); rc || !use)
+        return rc;
+    Bgzf &b = ctx->bgzf;
     int mod4 = line_mod4;
-    int64_t done = 0, written = 0;
-    while (done < use) {
-        const int64_t len = std::min(use - done, kBgzfPassChunks * BB_BGZF_CHUNK);
-        const int nc = (int)((len + BB_BGZF_CHUNK - 1) / BB_BGZF_CHUNK);
-        BB_CUDA(ctx, ctx->bgzf_in.ensure((size_t)len));
-        BB_CUDA(ctx, ctx->bgzf_slots.ensure((size_t)nc * 65536));
-        BB_CUDA(ctx, ctx->bgzf_lines.ensure((size_t)nc * sizeof(int32_t)));
-        BB_CUDA(ctx, ctx->bgzf_sizes.ensure((size_t)nc * sizeof(int32_t)));
-        BB_CUDA(ctx, ctx->bgzf_pref.ensure((size_t)(nc + 1) * sizeof(int64_t)));
-        BB_CUDA(ctx, ctx->bgzf_off.ensure((size_t)(nc + 1) * sizeof(int64_t)));
-        BB_CUDA(ctx, ctx->bgzf_out.ensure((size_t)bb_bgzf_bound(len)));
-        BB_CUDA(ctx, cudaMemcpyAsync(ctx->bgzf_in.p, in + done, (size_t)len, cudaMemcpyHostToDevice, st));
-        bbl_bgzf_pass(st, ctx->bgzf_in.as<uint8_t>(), len, nc, mod4, ctx->bgzf_lines.as<int32_t>(), ctx->bgzf_pref.as<int64_t>(),
-                      ctx->bgzf_slots.as<uint8_t>(), ctx->bgzf_sizes.as<int32_t>(), ctx->bgzf_off.as<int64_t>(),
-                      ctx->bgzf_out.as<uint8_t>());
-        BB_CUDA(ctx, cudaGetLastError());
-        BB_CUDA(ctx, cudaMemcpyAsync(ctx->h_bgzf, ctx->bgzf_pref.as<int64_t>() + nc, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-        BB_CUDA(ctx, cudaMemcpyAsync(ctx->h_bgzf + 1, ctx->bgzf_off.as<int64_t>() + nc, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-        BB_CUDA(ctx, cudaStreamSynchronize(st));
-        const int64_t bytes = ctx->h_bgzf[1];
-        if (bytes <= 0 || bytes > bb_bgzf_bound(len))
-            return set_err(ctx, BB_ERR_INTERNAL, "bb_bgzf_compress: members of " + std::to_string(bytes) + " bytes");
-        BB_CUDA(ctx, cudaMemcpyAsync(out + written, ctx->bgzf_out.p, (size_t)bytes, cudaMemcpyDeviceToHost, st));
-        BB_CUDA(ctx, cudaStreamSynchronize(st));
-        mod4 = (int)(ctx->h_bgzf[0] & 3);
-        written += bytes;
-        done += len;
-    }
-    *n_out = written;
-    *n_consumed = use;
-    return BB_OK;
+    // each pass also reads back the line index of its end (line_pref[n_chunks]): the next pass starts there
+    const int rc = bgzf_passes(ctx, "bb_bgzf_compress", use, out, n_out, [&](int64_t done, int64_t len, int nc) {
+        if (done) mod4 = (int)(b.h[0] & 3);
+        BB_CUDA(ctx, b.in.ensure((size_t)len));
+        BB_CUDA(ctx, b.lines.ensure((size_t)nc * sizeof(int32_t)));
+        BB_CUDA(ctx, b.pref.ensure((size_t)(nc + 1) * sizeof(int64_t)));
+        BB_CUDA(ctx, cudaMemcpyAsync(b.in.p, in + done, (size_t)len, cudaMemcpyHostToDevice, b.stream));
+        bbl_bgzf_pass(b.stream, b.in.as<uint8_t>(), len, nc, mod4, b.lines.as<int32_t>(), b.pref.as<int64_t>(),
+                      b.slots.as<uint8_t>(), b.sizes.as<int32_t>(), b.off.as<int64_t>(), b.out.as<uint8_t>());
+        BB_CUDA(ctx, cudaMemcpyAsync(b.h, b.pref.as<int64_t>() + nc, sizeof(int64_t), cudaMemcpyDeviceToHost, b.stream));
+        return BB_OK;
+    });
+    if (!rc) *n_consumed = use;
+    return rc;
 }
 
 // Enqueues the device-to-host copies of a finished (or at least scanned) worker's packed block on its stream.
@@ -1549,49 +1577,13 @@ extern "C" int bb_sequence_batch(bb_ctx *ctx, int32_t n_reads, const uint64_t *r
 }
 
 // ---- BAM output: records built on the device, compressed by the BGZF compressor --------------------------
-// Passes of bgzf_k_compress_bam over use bytes of a record stream starting at byte stream_base: from the device buffer
-// d_in, or from host memory h_in (then copied to bgzf_in pass by pass).  Members to out (capacity checked by the caller).
-static int bam_passes(bb_ctx *ctx, const uint8_t *h_in, const uint8_t *d_in, int64_t use, int64_t stream_base,
-                      const int64_t *d_fields, int64_t n_fields, uint8_t *out, int64_t *n_out) {
-    const cudaStream_t st = ctx->bgzf_stream;
-    int64_t done = 0, written = 0;
-    while (done < use) {
-        const int64_t len = std::min(use - done, kBgzfPassChunks * BB_BGZF_CHUNK);
-        const int nc = (int)((len + BB_BGZF_CHUNK - 1) / BB_BGZF_CHUNK);
-        BB_CUDA(ctx, ctx->bgzf_slots.ensure((size_t)nc * 65536));
-        BB_CUDA(ctx, ctx->bgzf_sizes.ensure((size_t)nc * sizeof(int32_t)));
-        BB_CUDA(ctx, ctx->bgzf_off.ensure((size_t)(nc + 1) * sizeof(int64_t)));
-        BB_CUDA(ctx, ctx->bgzf_out.ensure((size_t)bb_bgzf_bound(len)));
-        const uint8_t *src = d_in ? d_in + done : nullptr;
-        if (!src) {
-            BB_CUDA(ctx, ctx->bgzf_in.ensure((size_t)len));
-            BB_CUDA(ctx, cudaMemcpyAsync(ctx->bgzf_in.p, h_in + done, (size_t)len, cudaMemcpyHostToDevice, st));
-            src = ctx->bgzf_in.as<uint8_t>();
-        }
-        bbl_bgzf_pass_bam(st, src, len, nc, d_fields, n_fields, stream_base + done, ctx->bgzf_slots.as<uint8_t>(),
-                          ctx->bgzf_sizes.as<int32_t>(), ctx->bgzf_off.as<int64_t>(), ctx->bgzf_out.as<uint8_t>());
-        BB_CUDA(ctx, cudaGetLastError());
-        BB_CUDA(ctx, cudaMemcpyAsync(ctx->h_bgzf + 1, ctx->bgzf_off.as<int64_t>() + nc, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-        BB_CUDA(ctx, cudaStreamSynchronize(st));
-        const int64_t bytes = ctx->h_bgzf[1];
-        if (bytes <= 0 || bytes > bb_bgzf_bound(len))
-            return set_err(ctx, BB_ERR_INTERNAL, "BAM compressor: members of " + std::to_string(bytes) + " bytes");
-        BB_CUDA(ctx, cudaMemcpyAsync(out + written, ctx->bgzf_out.p, (size_t)bytes, cudaMemcpyDeviceToHost, st));
-        BB_CUDA(ctx, cudaStreamSynchronize(st));
-        written += bytes;
-        done += len;
-    }
-    *n_out = written;
-    return BB_OK;
-}
-
 // Makes the current buffer of `pair` (index cur) hold at least `bytes`: when it is too small, its first `keep` bytes move
 // to the other buffer, which becomes the current one.
 static int grow_keep(bb_ctx *ctx, DevBuf (&pair)[2], int &cur, size_t bytes, size_t keep) {
     if (bytes <= pair[cur].cap) return BB_OK;
     BB_CUDA(ctx, pair[1 - cur].ensure(bytes));
-    if (keep) BB_CUDA(ctx, cudaMemcpyAsync(pair[1 - cur].p, pair[cur].p, keep, cudaMemcpyDeviceToDevice, ctx->bgzf_stream));
-    BB_CUDA(ctx, cudaStreamSynchronize(ctx->bgzf_stream));
+    if (keep) BB_CUDA(ctx, cudaMemcpyAsync(pair[1 - cur].p, pair[cur].p, keep, cudaMemcpyDeviceToDevice, ctx->bgzf.stream));
+    BB_CUDA(ctx, cudaStreamSynchronize(ctx->bgzf.stream));
     pair[cur].release();
     cur = 1 - cur;
     return BB_OK;
@@ -1620,8 +1612,8 @@ extern "C" int bb_bam_build(bb_ctx *ctx, int32_t n, const bb_bam_record *recs, c
         at += size[(size_t)i];
     }
     BB_CUDA(ctx, cudaSetDevice(ctx->device));
-    if (int rc = ensure_bgzf_stream(ctx)) return rc;
-    const cudaStream_t st = ctx->bgzf_stream;
+    BB_CUDA(ctx, ctx->bgzf.open());
+    const cudaStream_t st = ctx->bgzf.stream;
     const size_t nf = ctx->bam_field_off.size();
     if (int rc = grow_keep(ctx, ctx->bam_buf, ctx->bam_cur, (size_t)std::max<int64_t>(at, 1), (size_t)ctx->bam_len)) return rc;
     if (int rc = grow_keep(ctx, ctx->bam_fields, ctx->bam_fcur, (nf + 2 * (size_t)n + 1) * 2 * sizeof(int64_t),
@@ -1658,19 +1650,19 @@ extern "C" int bb_bam_build(bb_ctx *ctx, int32_t n, const bb_bam_record *recs, c
 extern "C" int bb_bam_compress_device(bb_ctx *ctx, int final, uint8_t *out, int64_t out_cap, int64_t *n_out) {
     if (!ctx) return BB_ERR_ARG;
     if (out_cap < 0 || !n_out) return set_err(ctx, BB_ERR_ARG, "bb_bam_compress_device: bad arguments");
-    const int64_t use = final ? ctx->bam_len : ctx->bam_len / BB_BGZF_CHUNK * BB_BGZF_CHUNK;
-    *n_out = 0;
-    if (bb_bgzf_bound(use) > out_cap || (use && !out)) {
-        *n_out = bb_bgzf_bound(use);
-        return set_err(ctx, BB_ERR_CAPACITY, "bb_bam_compress_device: out_cap is less than bb_bgzf_bound of the input");
-    }
-    if (!use) return BB_OK;
-    BB_CUDA(ctx, cudaSetDevice(ctx->device));
-    if (int rc = ensure_bgzf_stream(ctx)) return rc;
+    int64_t use;
+    if (const int rc = bgzf_begin(ctx, "bb_bam_compress_device", ctx->bam_len, final, out, out_cap, n_out, nullptr, &use);
+        rc || !use)
+        return rc;
+    Bgzf &b = ctx->bgzf;
     const int cur = ctx->bam_cur, fcur = ctx->bam_fcur;
     const int64_t nf = (int64_t)ctx->bam_field_off.size();
-    if (int rc = bam_passes(ctx, nullptr, ctx->bam_buf[cur].as<uint8_t>(), use, ctx->bam_base, ctx->bam_fields[fcur].as<int64_t>(),
-                            nf, out, n_out))
+    if (const int rc = bgzf_passes(ctx, "bb_bam_compress_device", use, out, n_out, [&](int64_t done, int64_t len, int nc) {
+            bbl_bgzf_pass_bam(b.stream, ctx->bam_buf[cur].as<uint8_t>() + done, len, nc, ctx->bam_fields[fcur].as<int64_t>(), nf,
+                              ctx->bam_base + done, b.slots.as<uint8_t>(), b.sizes.as<int32_t>(), b.off.as<int64_t>(),
+                              b.out.as<uint8_t>());
+            return BB_OK;
+        }))
         return rc;
     // the rest (less than a chunk) and the fields that start in it move to the front of the other buffers
     const int64_t rest = ctx->bam_len - use, new_base = ctx->bam_base + use;
@@ -1680,10 +1672,10 @@ extern "C" int bb_bam_compress_device(bb_ctx *ctx, int final, uint8_t *out, int6
     BB_CUDA(ctx, ctx->bam_buf[1 - cur].ensure((size_t)std::max<int64_t>(rest, 1)));
     BB_CUDA(ctx, ctx->bam_fields[1 - fcur].ensure((size_t)std::max<int64_t>(nk, 1) * 2 * sizeof(int64_t)));
     if (rest) BB_CUDA(ctx, cudaMemcpyAsync(ctx->bam_buf[1 - cur].p, ctx->bam_buf[cur].as<uint8_t>() + use, (size_t)rest,
-                                           cudaMemcpyDeviceToDevice, ctx->bgzf_stream));
+                                           cudaMemcpyDeviceToDevice, b.stream));
     if (nk) BB_CUDA(ctx, cudaMemcpyAsync(ctx->bam_fields[1 - fcur].p, ctx->bam_fields[fcur].as<int64_t>() + 2 * keep_from,
-                                         (size_t)nk * 2 * sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->bgzf_stream));
-    BB_CUDA(ctx, cudaStreamSynchronize(ctx->bgzf_stream));
+                                         (size_t)nk * 2 * sizeof(int64_t), cudaMemcpyDeviceToDevice, b.stream));
+    BB_CUDA(ctx, cudaStreamSynchronize(b.stream));
     ctx->bam_cur = 1 - cur;
     ctx->bam_fcur = 1 - fcur;
     ctx->bam_field_off.erase(ctx->bam_field_off.begin(), ctx->bam_field_off.begin() + keep_from);
@@ -1717,8 +1709,8 @@ extern "C" int bb_bam_fetch_records(bb_ctx *ctx, const int64_t *dst_off, uint8_t
     }
     if (bytes) {
         BB_CUDA(ctx, cudaMemcpyAsync(ctx->h_bam, ctx->bam_buf[ctx->bam_cur].as<uint8_t>() + from, (size_t)bytes,
-                                     cudaMemcpyDeviceToHost, ctx->bgzf_stream));
-        BB_CUDA(ctx, cudaStreamSynchronize(ctx->bgzf_stream));
+                                     cudaMemcpyDeviceToHost, ctx->bgzf.stream));
+        BB_CUDA(ctx, cudaStreamSynchronize(ctx->bgzf.stream));
     }
     for (size_t i = 0; i < n; i++) {
         const int64_t at = ctx->bam_last_pos[i] - from;
@@ -1738,23 +1730,23 @@ extern "C" int bb_bam_compress(bb_ctx *ctx, const uint8_t *in, int64_t n, int64_
     for (int64_t i = 0; i < n_fields; i++)   // block starts must come in order, at least a field apart
         if (fields[2 * i + 1] < 0 || (i && fields[2 * i - 2] + fields[2 * i - 1] > fields[2 * i]))
             return set_err(ctx, BB_ERR_ARG, "bb_bam_compress: fields overlap or are out of order");
-    const int64_t use = final ? n : n / BB_BGZF_CHUNK * BB_BGZF_CHUNK;
-    *n_out = 0;
-    *n_consumed = 0;
-    if (bb_bgzf_bound(use) > out_cap || (use && !out)) {
-        *n_out = bb_bgzf_bound(use);
-        return set_err(ctx, BB_ERR_CAPACITY, "bb_bam_compress: out_cap is less than bb_bgzf_bound of the input");
-    }
-    if (!use) return BB_OK;
-    BB_CUDA(ctx, cudaSetDevice(ctx->device));
-    if (int rc = ensure_bgzf_stream(ctx)) return rc;
+    int64_t use;
+    if (const int rc = bgzf_begin(ctx, "bb_bam_compress", n, final, out, out_cap, n_out, n_consumed, &use); rc || !use)
+        return rc;
+    Bgzf &b = ctx->bgzf;
     int64_t f0 = 0, f1 = n_fields;   // the fields that start inside in[0 .. use)
     while (f0 < n_fields && fields[2 * f0] < stream_base) f0++;
     while (f1 > f0 && fields[2 * (f1 - 1)] >= stream_base + use) f1--;
-    if (int rc = upload(ctx, ctx->bgzf_stream, ctx->bam_hfields, fields + 2 * f0, (size_t)(f1 - f0) * 2)) return rc;
-    if (int rc = bam_passes(ctx, in, nullptr, use, stream_base, ctx->bam_hfields.as<int64_t>(), f1 - f0, out, n_out)) return rc;
-    *n_consumed = use;
-    return BB_OK;
+    if (int rc = upload(ctx, b.stream, ctx->bam_hfields, fields + 2 * f0, (size_t)(f1 - f0) * 2)) return rc;
+    const int rc = bgzf_passes(ctx, "bb_bam_compress", use, out, n_out, [&](int64_t done, int64_t len, int nc) {
+        BB_CUDA(ctx, b.in.ensure((size_t)len));
+        BB_CUDA(ctx, cudaMemcpyAsync(b.in.p, in + done, (size_t)len, cudaMemcpyHostToDevice, b.stream));
+        bbl_bgzf_pass_bam(b.stream, b.in.as<uint8_t>(), len, nc, ctx->bam_hfields.as<int64_t>(), f1 - f0, stream_base + done,
+                          b.slots.as<uint8_t>(), b.sizes.as<int32_t>(), b.off.as<int64_t>(), b.out.as<uint8_t>());
+        return BB_OK;
+    });
+    if (!rc) *n_consumed = use;
+    return rc;
 }
 
 // ---- single-pair entry points (worker 0's stream and scratch) ----------------------------------------------

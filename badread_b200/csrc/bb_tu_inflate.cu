@@ -21,16 +21,43 @@ struct DevBuf {   // released on every exit path
     ~DevBuf() { if (p) cudaFree(p); }
 };
 
-int cuda_fail(const char *what, cudaError_t e) {
-    char msg[256];
-    std::snprintf(msg, sizeof(msg), "bb_bgzf_decompress: %s: %s", what, cudaGetErrorString(e));
-    bbm_set_error(msg);
+int cuda_fail(const char *what, cudaError_t e, char *msg, size_t msg_len) {
+    std::snprintf(msg, msg_len, "bb_bgzf_decompress: %s: %s", what, cudaGetErrorString(e));
     return BB_ERR_CUDA;
 }
 
 }  // namespace
 
-#define BBI_TRY(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return cuda_fail(#call, e_); } while (0)
+#define BBI_TRY(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return cuda_fail(#call, e_, msg, msg_len); } while (0)
+
+// The device step after infl_walk: uploads the input and its members, inflates them on `st` and checks every member's
+// status.  On success *out is a device buffer of `total` bytes (16 when total is 0) that the caller frees; otherwise
+// msg says why (a corrupt member by index and offset).
+static int infl_device(cudaStream_t st, const uint8_t *in, int64_t n, const std::vector<InflMember> &members, int64_t total,
+                       uint8_t **out, char *msg, size_t msg_len) {
+    DevBuf d_in, d_out, d_members, d_status;
+    BBI_TRY(cudaMalloc(&d_out.p, (size_t)(total ? total : 16)));
+    if (!members.empty()) {
+        const int64_t n_members = (int64_t)members.size();
+        BBI_TRY(cudaMalloc(&d_in.p, (size_t)n));
+        BBI_TRY(cudaMalloc(&d_members.p, members.size() * sizeof(InflMember)));
+        BBI_TRY(cudaMalloc(&d_status.p, members.size() * sizeof(int32_t)));
+        BBI_TRY(cudaMemcpyAsync(d_in.p, in, (size_t)n, cudaMemcpyHostToDevice, st));
+        BBI_TRY(cudaMemcpyAsync(d_members.p, members.data(), members.size() * sizeof(InflMember), cudaMemcpyHostToDevice, st));
+        (void)cudaGetLastError();   // (report this call's launch only)
+        const int64_t grid = (n_members + INFL_WARPS - 1) / INFL_WARPS;
+        infl_k_members<<<(unsigned)grid, INFL_THREADS, 0, st>>>((const uint8_t *)d_in.p, (const InflMember *)d_members.p,
+                                                                 n_members, (uint8_t *)d_out.p, (int32_t *)d_status.p);
+        BBI_TRY(cudaGetLastError());
+        std::vector<int32_t> status(members.size());
+        BBI_TRY(cudaMemcpyAsync(status.data(), d_status.p, members.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        BBI_TRY(cudaStreamSynchronize(st));
+        if (infl_first_failure(members, status.data(), msg, msg_len)) return BB_ERR_ARG;
+    }
+    *out = (uint8_t *)d_out.p;
+    d_out.p = nullptr;
+    return BB_OK;
+}
 
 extern "C" int bb_bgzf_decompress(int device, const uint8_t *in, int64_t n, uint8_t *out, int64_t out_cap, int64_t *n_out) {
     bbm_set_error("");
@@ -46,35 +73,22 @@ extern "C" int bb_bgzf_decompress(int device, const uint8_t *in, int64_t n, uint
         return BB_ERR_ARG;
     }
     *n_out = total;
-    if (total > out_cap) {
+    if (total > out_cap) {   // (answered from the host walk: the caller asks again with the room)
         std::snprintf(msg, sizeof(msg), "bb_bgzf_decompress: %lld bytes of output, capacity %lld", (long long)total,
                       (long long)out_cap);
         bbm_set_error(msg);
         return BB_ERR_CAPACITY;
     }
     if (members.empty()) return BB_OK;
-    const int64_t n_members = (int64_t)members.size();
-    BBI_TRY(cudaSetDevice(device));
-    (void)cudaGetLastError();   // (report this call's launch only)
-    DevBuf d_in, d_out, d_members, d_status;
-    BBI_TRY(cudaMalloc(&d_in.p, (size_t)n));
-    BBI_TRY(cudaMalloc(&d_out.p, (size_t)(total ? total : 16)));
-    BBI_TRY(cudaMalloc(&d_members.p, members.size() * sizeof(InflMember)));
-    BBI_TRY(cudaMalloc(&d_status.p, members.size() * sizeof(int32_t)));
-    BBI_TRY(cudaMemcpy(d_in.p, in, (size_t)n, cudaMemcpyHostToDevice));
-    BBI_TRY(cudaMemcpy(d_members.p, members.data(), members.size() * sizeof(InflMember), cudaMemcpyHostToDevice));
-    const int64_t grid = (n_members + INFL_WARPS - 1) / INFL_WARPS;
-    infl_k_members<<<(unsigned)grid, INFL_THREADS>>>((const uint8_t *)d_in.p, (const InflMember *)d_members.p, n_members,
-                                                      (uint8_t *)d_out.p, (int32_t *)d_status.p);
-    BBI_TRY(cudaGetLastError());
-    std::vector<int32_t> status(members.size());
-    BBI_TRY(cudaMemcpy(status.data(), d_status.p, members.size() * sizeof(int32_t), cudaMemcpyDeviceToHost));
-    if (infl_first_failure(members, status.data(), msg, sizeof(msg))) {
-        bbm_set_error(msg);
-        return BB_ERR_ARG;
-    }
-    BBI_TRY(cudaMemcpy(out, d_out.p, (size_t)total, cudaMemcpyDeviceToHost));
-    return BB_OK;
+    uint8_t *d_out = nullptr;
+    cudaError_t e = cudaSetDevice(device);
+    int rc = e == cudaSuccess ? infl_device(0, in, n, members, total, &d_out, msg, sizeof(msg))
+                              : cuda_fail("cudaSetDevice", e, msg, sizeof(msg));
+    if (rc == BB_OK && (e = cudaMemcpy(out, d_out, (size_t)total, cudaMemcpyDeviceToHost)) != cudaSuccess)
+        rc = cuda_fail("cudaMemcpy", e, msg, sizeof(msg));
+    cudaFree(d_out);
+    if (rc) bbm_set_error(msg);
+    return rc;
 }
 
 int bbl_bgzf_inflate_device(cudaStream_t st, const uint8_t *in, int64_t n, uint8_t **out, int64_t *total, char *msg,
@@ -83,35 +97,5 @@ int bbl_bgzf_inflate_device(cudaStream_t st, const uint8_t *in, int64_t n, uint8
     *total = 0;
     std::vector<InflMember> members;
     if (!infl_walk(in, n, members, total, msg, msg_len)) return BB_ERR_ARG;
-    auto fail = [&](const char *what, cudaError_t e) {
-        std::snprintf(msg, msg_len, "%s: %s", what, cudaGetErrorString(e));
-        return BB_ERR_CUDA;
-    };
-    DevBuf d_in, d_members, d_status, d_out;
-    cudaError_t e;
-    if ((e = cudaMalloc(&d_out.p, (size_t)(*total ? *total : 16))) != cudaSuccess) return fail("cudaMalloc", e);
-    if (!members.empty()) {
-        const int64_t n_members = (int64_t)members.size();
-        if ((e = cudaMalloc(&d_in.p, (size_t)n)) != cudaSuccess ||
-            (e = cudaMalloc(&d_members.p, members.size() * sizeof(InflMember))) != cudaSuccess ||
-            (e = cudaMalloc(&d_status.p, members.size() * sizeof(int32_t))) != cudaSuccess)
-            return fail("cudaMalloc", e);
-        if ((e = cudaMemcpyAsync(d_in.p, in, (size_t)n, cudaMemcpyHostToDevice, st)) != cudaSuccess ||
-            (e = cudaMemcpyAsync(d_members.p, members.data(), members.size() * sizeof(InflMember), cudaMemcpyHostToDevice,
-                                 st)) != cudaSuccess)
-            return fail("cudaMemcpyAsync", e);
-        const int64_t grid = (n_members + INFL_WARPS - 1) / INFL_WARPS;
-        infl_k_members<<<(unsigned)grid, INFL_THREADS, 0, st>>>((const uint8_t *)d_in.p, (const InflMember *)d_members.p,
-                                                                 n_members, (uint8_t *)d_out.p, (int32_t *)d_status.p);
-        if ((e = cudaGetLastError()) != cudaSuccess) return fail("infl_k_members", e);
-        std::vector<int32_t> status(members.size());
-        if ((e = cudaMemcpyAsync(status.data(), d_status.p, members.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, st)) !=
-                cudaSuccess ||
-            (e = cudaStreamSynchronize(st)) != cudaSuccess)
-            return fail("infl_k_members", e);
-        if (infl_first_failure(members, status.data(), msg, msg_len)) return BB_ERR_ARG;
-    }
-    *out = (uint8_t *)d_out.p;
-    d_out.p = nullptr;
-    return BB_OK;
+    return infl_device(st, in, n, members, *total, out, msg, msg_len);
 }

@@ -5,6 +5,7 @@ No PyTorch, no CPU path: construction fails when the library or a GPU is missing
 """
 import ctypes
 import os
+import threading
 
 import numpy as np
 
@@ -26,6 +27,15 @@ class EngineError(RuntimeError):
 
 def _ptr(a):
     return a.ctypes.data_as(ctypes.c_void_p) if a is not None else None
+
+
+def _host_alloc(nbytes):
+    """nbytes of page-locked memory (bb_host_alloc), so that copies between it and the GPUs run at the link's rate:
+    (handle for bb_host_free, uint8 array over the bytes)."""
+    p = ctypes.c_void_p()
+    if _lib.lib().bb_host_alloc(ctypes.byref(p), nbytes) != 0:
+        raise EngineError(f'bb_host_alloc({nbytes}) failed')
+    return p, np.ctypeslib.as_array((ctypes.c_uint8 * nbytes).from_address(p.value))
 
 
 class FragmentBatch(object):
@@ -120,11 +130,8 @@ class FastaFile(object):
                 self.data = np.frombuffer(f.read(), dtype=np.uint8)
             return
         size = os.path.getsize(filename)
-        p = ctypes.c_void_p()
-        if self._lib.bb_host_alloc(ctypes.byref(p), max(size, 1)) != 0:
-            raise EngineError(f'bb_host_alloc({size}) failed')
-        self._pinned = p
-        self.data = np.ctypeslib.as_array((ctypes.c_uint8 * max(size, 1)).from_address(p.value))[:size]
+        self._pinned, data = _host_alloc(max(size, 1))
+        self.data = data[:size]
         view, got = memoryview(self.data), 0
         with open(filename, 'rb', buffering=0) as f:
             while got < size:
@@ -290,12 +297,10 @@ class Engine(object):
             cap = int(cap * 1.25) + 4096
             # earlier (smaller) buffers stay allocated until close(): BatchResults handed out before still view them
             bufs = []
-            for _ in range(2):  # page-locked, so that the device-to-host copies run at link rate
-                p = ctypes.c_void_p()
-                if self._lib.bb_host_alloc(ctypes.byref(p), cap) != 0:
-                    raise EngineError(f'bb_host_alloc({cap}) failed')
+            for _ in range(2):
+                p, buf = _host_alloc(cap)
                 self._pinned.append(p)
-                bufs.append(np.ctypeslib.as_array((ctypes.c_uint8 * cap).from_address(p.value)))
+                bufs.append(buf)
             self._seq_buf, self._qual_buf = bufs
             self._out_cap = cap
 
@@ -398,19 +403,12 @@ class Engine(object):
         are compressed.  Returns (members, bytes of buf consumed); members is a uint8 array in page-locked memory that the
         next call reuses.  The end-of-file member is not included (badread_b200.bgzf.EOF_MEMBER)."""
         data = np.frombuffer(buf, dtype=np.uint8)
-        need = int(self._lib.bb_bgzf_bound(data.size))
-        if self._bgzf_buf is None or self._bgzf_buf.size < need:
-            cap = max(need + need // 8, 1 << 20)
-            p = ctypes.c_void_p()
-            if self._lib.bb_host_alloc(ctypes.byref(p), cap) != 0:
-                raise EngineError(f'bb_host_alloc({cap}) failed')
-            self._pinned.append(p)
-            self._bgzf_buf = np.ctypeslib.as_array((ctypes.c_uint8 * cap).from_address(p.value))
+        buf_out = self._members_buf(int(self._lib.bb_bgzf_bound(data.size)))
         n_out, n_used = ctypes.c_int64(0), ctypes.c_int64(0)
         rc = self._lib.bb_bgzf_compress(self._ctx, _ptr(data) if data.size else None, data.size, int(line_mod4), int(bool(final)),
-                                        _ptr(self._bgzf_buf), self._bgzf_buf.size, ctypes.byref(n_out), ctypes.byref(n_used))
+                                        _ptr(buf_out), buf_out.size, ctypes.byref(n_out), ctypes.byref(n_used))
         self._check(rc, 'bb_bgzf_compress')
-        return self._bgzf_buf[:n_out.value], int(n_used.value)
+        return buf_out[:n_out.value], int(n_used.value)
 
     # ---- BAM output (badread_b200/bam.py)
     def run_batch_results(self, batch):
@@ -433,13 +431,10 @@ class Engine(object):
                                            _ptr(text) if text.size else None, text.size), 'bb_bam_build')
 
     def _members_buf(self, need):
+        """The page-locked buffer the compressors write members to, grown to at least `need` bytes."""
         if self._bgzf_buf is None or self._bgzf_buf.size < need:
-            cap = max(need + need // 8, 1 << 20)
-            p = ctypes.c_void_p()
-            if self._lib.bb_host_alloc(ctypes.byref(p), cap) != 0:
-                raise EngineError(f'bb_host_alloc({cap}) failed')
+            p, self._bgzf_buf = _host_alloc(max(need + need // 8, 1 << 20))
             self._pinned.append(p)
-            self._bgzf_buf = np.ctypeslib.as_array((ctypes.c_uint8 * cap).from_address(p.value))
         return self._bgzf_buf
 
     def bam_compress_device(self, final=False):
@@ -534,6 +529,30 @@ def comm_init_all(engines):
     if rc != 0:
         msg = _lib.lib().bb_last_error(engines[0]._ctx)
         raise EngineError(f'bb_comm_init_all failed ({rc}): {msg.decode() if msg else ""}')
+
+
+def run_each(n, work):
+    """work(k) for k < n, one host thread each when n > 1 (inline when n == 1).  Every call finishes before the exception
+    of the lowest k that raised one is re-raised on the caller's thread."""
+    errors = [None] * n
+
+    def run(k):
+        try:
+            work(k)
+        except BaseException as e:
+            errors[k] = e
+
+    if n == 1:
+        run(0)
+    else:
+        threads = [threading.Thread(target=run, args=(k,)) for k in range(n)]
+        for t in threads:
+            t.start()
+        for t in threads:
+            t.join()
+    for e in errors:
+        if e is not None:
+            raise e
 
 
 def allreduce_bases_all(engines, local):

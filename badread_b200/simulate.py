@@ -22,13 +22,12 @@ reference's interface and is distributed under the same licence (see LICENSE and
 import random
 import statistics
 import sys
-import threading
 import uuid
 
 import numpy as np
 
 from . import settings
-from .engine import Engine, FastaFile, FragmentBatch, default_engine, next_read_index
+from .engine import Engine, FastaFile, FragmentBatch, default_engine, next_read_index, run_each
 from .error_model import ErrorModel
 from .fragment_lengths import FragmentLengths
 from .identities import Identities
@@ -98,27 +97,15 @@ class DeviceReference(Reference):
         print('', file=output)
         print(f'Loading reference from {filename}', file=output)
         fasta = FastaFile(filename)
+        tables = [None] * len(engines)
+
+        def load(g):
+            tables[g] = engines[g].load_fasta(fasta)
+
         try:
-            tables = [None] * len(engines)
-            errors = [None] * len(engines)
-
-            def load(g):
-                try:
-                    tables[g] = engines[g].load_fasta(fasta)
-                except BaseException as e:   # re-raised on the main thread
-                    errors[g] = e
-
-            threads = [threading.Thread(target=load, args=(g,)) for g in range(1, len(engines))]
-            for t in threads:
-                t.start()
-            load(0)
-            for t in threads:
-                t.join()
+            run_each(len(engines), load)
         finally:
             fasta.close()
-        for e in errors:
-            if e is not None:
-                raise e
         self.names, self.lengths, depths, circular, left_hairpin, right_hairpin = tables[0]
         self.depths = [depths[n] for n in self.names]
         self.circular = [circular[n] for n in self.names]
@@ -575,32 +562,19 @@ def run_batches(args, ref, frag_lengths, identities, error_model, qscore_model, 
         while total_size < target_size:
             want = int((target_size - total_size) / mean_len * 1.05) + 8
             n_batch = max(1, min(max_batch, want))
-            planned, results, errors = [None] * n_gpus, [None] * n_gpus, [None] * n_gpus
+            planned, results = [None] * n_gpus, [None] * n_gpus
 
             def work(g):
-                try:
-                    n_g = len(range(g, n_batch, n_gpus))
-                    planned[g] = planners[g].plan(next_index + g, n_g, stride=n_gpus)
-                    if not n_g:
-                        results[g] = None
-                    elif bam:
-                        results[g] = engines[g].run_batch_results(planned[g])[0]
-                    else:
-                        results[g] = engines[g].sequence_batch(planned[g])[0]
-                except BaseException as e:   # re-raised on the main thread (a worker thread would swallow it)
-                    errors[g] = e
+                n_g = len(range(g, n_batch, n_gpus))
+                planned[g] = planners[g].plan(next_index + g, n_g, stride=n_gpus)
+                if not n_g:
+                    results[g] = None
+                elif bam:
+                    results[g] = engines[g].run_batch_results(planned[g])[0]
+                else:
+                    results[g] = engines[g].sequence_batch(planned[g])[0]
 
-            if n_gpus == 1:
-                work(0)
-            else:
-                threads = [threading.Thread(target=work, args=(g,)) for g in range(n_gpus)]
-                for t in threads:
-                    t.start()
-                for t in threads:
-                    t.join()
-            for e in errors:
-                if e is not None:
-                    raise e
+            run_each(n_gpus, work)
             recs = [r.records if r is not None else (ReadResult * 1)() for r in results]
             if bam:
                 n_emit, bases = writer.write_batch(planned, recs, total_size, target_size)
