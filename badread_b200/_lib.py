@@ -45,6 +45,15 @@ class BamRecord(ctypes.Structure):
                 ('name_len', ctypes.c_int32), ('co_len', ctypes.c_int32), ('reserved', ctypes.c_int32)]
 
 
+class GzipStats(ctypes.Structure):
+    """bb_gzip_stats (include/badread_b200.h)."""
+    _fields_ = [(f, ctypes.c_int64) for f in ('members', 'chunks', 'absorbed', 'first_candidate', 'repaired', 'chained',
+                                              'reruns')] + [('bgzf', ctypes.c_int32), ('reserved', ctypes.c_int32)]
+
+    def as_dict(self):
+        return {f: int(getattr(self, f)) for f, _ in self._fields_ if f != 'reserved'}
+
+
 class PlanConfig(ctypes.Structure):
     """bb_plan_config (include/badread_b200.h)."""
     _fields_ = [('seed', ctypes.c_uint64), ('n_contigs', ctypes.c_int32), ('contig_len', ctypes.c_void_p),
@@ -106,6 +115,7 @@ def lib():
         'bb_upload_reference': (c.c_int, [vp, vp, i64]),
         'bb_fasta_parse': (c.c_int, [vp, vp, i64, c.c_int, P(i32), P(i64), P(i64)]),
         'bb_fasta_headers': (c.c_int, [vp, vp, i64, vp, vp, i32]),
+        'bb_last_gzip_stats': (c.c_int, [vp, P(GzipStats)]),
         'bb_fasta_reference': (c.c_int, [vp, i32, vp, vp]),
         'bb_download_reference': (c.c_int, [vp, i64, i64, vp]),
         'bb_upload_error_model': (c.c_int, [vp, c.c_int, c.c_int, vp, i64, i32, vp, vp, vp, vp, vp, i64]),
@@ -152,6 +162,7 @@ def lib():
         'bb_bgzf_bound': (i64, [i64]),
         'bb_bgzf_compress': (c.c_int, [vp, vp, i64, c.c_int, c.c_int, vp, i64, P(i64), P(i64)]),
         'bb_bgzf_decompress': (c.c_int, [c.c_int, vp, i64, vp, i64, P(i64)]),
+        'bb_gzip_decompress': (c.c_int, [c.c_int, vp, i64, vp, i64, P(i64), i64, P(GzipStats)]),
         'bb_fetch_last_batch_results': (c.c_int, [vp, vp, P(i64)]),
         'bb_bam_build': (c.c_int, [vp, i32, vp, vp, i64]),
         'bb_bam_compress_device': (c.c_int, [vp, c.c_int, vp, i64, P(i64)]),
@@ -183,4 +194,4 @@ EXPORTED_SYMBOLS = ['bb_create', 'bb_destroy', 'bb_last_error', 'bb_version', 'b
                     'bb_bgzf_bound', 'bb_bgzf_compress', 'bb_bgzf_decompress', 'bb_aln_parse', 'bb_aln_view_get', 'bb_aln_free',
                     'bb_fetch_last_batch_results', 'bb_bam_build', 'bb_bam_compress_device', 'bb_bam_fetch_records',
                     'bb_bam_compress', 'bb_bam_layout_sharded', 'bb_fasta_parse', 'bb_fasta_headers', 'bb_fasta_reference',
-                    'bb_download_reference']
+                    'bb_download_reference', 'bb_gzip_decompress', 'bb_last_gzip_stats']

@@ -7,7 +7,8 @@ writer carries the tail of every buffer into the next one, so the compressed byt
 on the number of GPUs.
 
 Input (`decompress`): a whole BGZF file, BAM for the model builders, inflated on one GPU, one warp per member
-(csrc/bb_inflate.cuh).
+(csrc/bb_inflate.cuh).  `gunzip` takes any gzip stream, BGZF or not: one that is not BGZF is decoded in parallel chunks
+(csrc/bb_gunzip.cuh).
 """
 import ctypes
 
@@ -38,6 +39,33 @@ def decompress(data, device=0):
     if rc != _lib.BB_OK:
         raise RuntimeError('bgzf.decompress: ' + L.bb_model_error().decode(errors='replace'))
     return out
+
+
+def gunzip(data, device=0, chunk_bytes=0):
+    """(the inflated bytes as a bytearray, the stats as a dict) of the gzip stream `data` (bytes-like, any number of
+    members, BGZF or not), inflated on GPU `device` (bb_gzip_decompress); chunk_bytes: compressed bytes per chunk, 0 for
+    the default.  Raises ValueError with the library's message for a corrupt stream (the member named by index and
+    offset)."""
+    L = _lib.lib()
+    src = np.frombuffer(memoryview(data).cast('B'), dtype=np.uint8)
+    src_ptr = src.ctypes.data_as(ctypes.c_void_p) if src.size else None
+    n_out, stats = ctypes.c_int64(0), _lib.GzipStats()
+    out = bytearray(4 * src.size)   # (a guess: a larger stream is inflated again into the room it asks for)
+
+    def call(buf):
+        ptr = (ctypes.c_char * len(buf)).from_buffer(buf) if buf else None
+        return L.bb_gzip_decompress(device, src_ptr, src.size, ptr, len(buf), ctypes.byref(n_out), chunk_bytes,
+                                    ctypes.byref(stats))
+    rc = call(out)
+    if rc == _lib.BB_ERR_CAPACITY:
+        out = bytearray(n_out.value)
+        rc = call(out)
+    if rc == _lib.BB_ERR_ARG:
+        raise ValueError(L.bb_model_error().decode(errors='replace'))
+    if rc != _lib.BB_OK:
+        raise RuntimeError('bgzf.gunzip: ' + L.bb_model_error().decode(errors='replace'))
+    del out[n_out.value:]
+    return out, stats.as_dict()
 
 
 def chunk_runs(n_chunks, n_engines):

@@ -215,6 +215,7 @@ struct bb_ctx {
     // a FASTA parsed by bb_fasta_parse (fa_n_kept >= 0): its kept bytes, header texts and each header's kept offset,
     // until bb_fasta_reference forms the reference from them
     DevBuf fa_kept; int64_t fa_n_kept = -1;
+    bb_gzip_stats gz_stats{};   // how the last bb_fasta_parse inflated its input
     std::string fa_text; std::vector<int64_t> fa_text_off, fa_kept_off;
     bool have_em = false, have_qm = false;
     BBErrorModelDev em{}; DevBuf em_k2r, em_rowoff, em_cum, em_flags, em_slots, em_pool, em_rowinfo;
@@ -458,6 +459,7 @@ extern "C" int bb_fasta_parse(bb_ctx *ctx, const uint8_t *data, int64_t n, int i
     BB_CUDA(ctx, cudaSetDevice(ctx->device));
     for (const auto &w : ctx->workers) BB_CUDA(ctx, cudaStreamSynchronize(w->stream));
     fasta_reset(ctx);
+    ctx->gz_stats = bb_gzip_stats{};
     ctx->ref.release();   // (replaced by bb_fasta_reference; freed first, so that the parse has its memory)
     ctx->ref_len = 0;
     const cudaStream_t st = ctx->w0().stream;
@@ -466,7 +468,8 @@ extern "C" int bb_fasta_parse(bb_ctx *ctx, const uint8_t *data, int64_t n, int i
     if (is_bgzf) {
         uint8_t *p = nullptr;
         char msg[256];
-        if (const int rc = bbl_bgzf_inflate_device(st, data, n, &p, &len, msg, sizeof(msg))) return set_err(ctx, rc, msg);
+        if (const int rc = bbl_gzip_inflate_device(st, data, n, 0, &p, &len, &ctx->gz_stats, msg, sizeof(msg)))
+            return set_err(ctx, rc, msg);
         text.p = p;
         text.cap = (size_t)std::max<int64_t>(len, 16);
     } else {
@@ -511,6 +514,12 @@ extern "C" int bb_fasta_parse(bb_ctx *ctx, const uint8_t *data, int64_t n, int i
     *n_headers = (int32_t)nh;
     *text_bytes = tlen;
     *n_kept = kept;
+    return BB_OK;
+}
+
+extern "C" int bb_last_gzip_stats(const bb_ctx *ctx, bb_gzip_stats *stats) {
+    if (!ctx || !stats) return BB_ERR_ARG;
+    *stats = ctx->gz_stats;
     return BB_OK;
 }
 

@@ -147,6 +147,53 @@ __device__ __forceinline__ bool infl_code_ok(const InflHuff &h, int err, int n) 
     return h.count[1] == 1 && n - h.count[0] == 1;
 }
 
+// The header of a dynamic Huffman block after its 3 type bits: the code-length code, the run-length coded code lengths
+// and the literal / length and distance codes built into s.lit and s.dist.  One thread.  Returns an InflStatus.  The
+// block finder of bb_gunzip.cuh holds candidate block starts to these same rules.
+__device__ __forceinline__ int infl_dynamic_tables(InflBits &b, InflWarpSmem &s) {
+    const int nlen = (int)infl_get(b, 5) + 257, ndist = (int)infl_get(b, 5) + 1, ncode = (int)infl_get(b, 4) + 4;
+    if (nlen > 286 || ndist > 30) return INFL_BAD_TABLE;
+    for (int i = 0; i < 19; i++) s.lens[infl_c_cl_order[i]] = i < ncode ? (uint8_t)infl_get(b, 3) : 0;
+    if (infl_past_end(b)) return INFL_TRUNCATED;
+    if (infl_build(s.lit, s.lens, 19) != 0) return INFL_BAD_TABLE;   // (the code-length code, complete)
+    for (int i = 0; i < nlen + ndist;) {
+        const int sym = infl_decode(b, s.lit);
+        if (sym < 0) return INFL_BAD_TABLE;
+        if (infl_past_end(b)) return INFL_TRUNCATED;
+        if (sym < 16) {
+            s.lens[i++] = (uint8_t)sym;
+            continue;
+        }
+        uint8_t v = 0;
+        int rep;
+        if (sym == 16) {
+            if (i == 0) return INFL_BAD_TABLE;
+            v = s.lens[i - 1];
+            rep = 3 + (int)infl_get(b, 2);
+        } else if (sym == 17) {
+            rep = 3 + (int)infl_get(b, 3);
+        } else {
+            rep = 11 + (int)infl_get(b, 7);
+        }
+        if (i + rep > nlen + ndist) return INFL_BAD_TABLE;
+        while (rep--) s.lens[i++] = v;
+    }
+    if (s.lens[256] == 0) return INFL_BAD_TABLE;  // no end-of-block code
+    int err = infl_build(s.lit, s.lens, nlen);
+    if (!infl_code_ok(s.lit, err, nlen)) return INFL_BAD_TABLE;
+    err = infl_build(s.dist, s.lens + nlen, ndist);
+    if (!infl_code_ok(s.dist, err, ndist)) return INFL_BAD_TABLE;   // (no distance codes at all: accepted)
+    return INFL_OK;
+}
+
+// The fixed Huffman codes (RFC 1951 §3.2.6) built into s.lit and s.dist.  One thread.
+__device__ __forceinline__ void infl_fixed_tables(InflWarpSmem &s) {
+    for (int i = 0; i < 288; i++) s.lens[i] = i < 144 ? 8 : i < 256 ? 9 : i < 280 ? 7 : 8;
+    infl_build(s.lit, s.lens, 288);
+    for (int i = 0; i < 30; i++) s.lens[i] = 5;
+    infl_build(s.dist, s.lens, 30);
+}
+
 // Inflates one member's deflate data in[0..n) into out[0..isize).  One thread.  Returns an InflStatus.
 __device__ int infl_member(const uint8_t *in, int32_t n, uint8_t *out, int32_t isize, InflWarpSmem &s) {
     InflBits b{in, n, 0, 0, 0};
@@ -167,43 +214,10 @@ __device__ int infl_member(const uint8_t *in, int32_t n, uint8_t *out, int32_t i
         }
         if (type == 3) return INFL_BAD_BLOCK;
         if (type == 1) {                                  // fixed Huffman codes
-            for (int i = 0; i < 288; i++) s.lens[i] = i < 144 ? 8 : i < 256 ? 9 : i < 280 ? 7 : 8;
-            infl_build(s.lit, s.lens, 288);
-            for (int i = 0; i < 30; i++) s.lens[i] = 5;
-            infl_build(s.dist, s.lens, 30);
+            infl_fixed_tables(s);
         } else {                                          // dynamic Huffman codes
-            const int nlen = (int)infl_get(b, 5) + 257, ndist = (int)infl_get(b, 5) + 1, ncode = (int)infl_get(b, 4) + 4;
-            if (nlen > 286 || ndist > 30) return INFL_BAD_TABLE;
-            for (int i = 0; i < 19; i++) s.lens[infl_c_cl_order[i]] = i < ncode ? (uint8_t)infl_get(b, 3) : 0;
-            if (infl_past_end(b)) return INFL_TRUNCATED;
-            if (infl_build(s.lit, s.lens, 19) != 0) return INFL_BAD_TABLE;   // (the code-length code, complete)
-            for (int i = 0; i < nlen + ndist;) {
-                const int sym = infl_decode(b, s.lit);
-                if (sym < 0) return INFL_BAD_TABLE;
-                if (infl_past_end(b)) return INFL_TRUNCATED;
-                if (sym < 16) {
-                    s.lens[i++] = (uint8_t)sym;
-                    continue;
-                }
-                uint8_t v = 0;
-                int rep;
-                if (sym == 16) {
-                    if (i == 0) return INFL_BAD_TABLE;
-                    v = s.lens[i - 1];
-                    rep = 3 + (int)infl_get(b, 2);
-                } else if (sym == 17) {
-                    rep = 3 + (int)infl_get(b, 3);
-                } else {
-                    rep = 11 + (int)infl_get(b, 7);
-                }
-                if (i + rep > nlen + ndist) return INFL_BAD_TABLE;
-                while (rep--) s.lens[i++] = v;
-            }
-            if (s.lens[256] == 0) return INFL_BAD_TABLE;  // no end-of-block code
-            int err = infl_build(s.lit, s.lens, nlen);
-            if (!infl_code_ok(s.lit, err, nlen)) return INFL_BAD_TABLE;
-            err = infl_build(s.dist, s.lens + nlen, ndist);
-            if (!infl_code_ok(s.dist, err, ndist)) return INFL_BAD_TABLE;   // (no distance codes at all: accepted)
+            const int st = infl_dynamic_tables(b, s);
+            if (st != INFL_OK) return st;
         }
         for (;;) {
             int sym = infl_decode(b, s.lit);
@@ -232,6 +246,7 @@ __device__ int infl_member(const uint8_t *in, int32_t n, uint8_t *out, int32_t i
     return pos == isize ? INFL_OK : INFL_SHORT;
 }
 
+#ifndef INFL_NO_MEMBER_KERNEL   // (bb_tu_gunzip.cu uses the decoder, not this kernel)
 // Member m = blockIdx.x * INFL_WARPS + warp: its deflate data in[members[m].data ..] inflated to out[members[m].out ..],
 // then its CRC-32 checked; status[m] = InflStatus.
 __global__ void __launch_bounds__(INFL_THREADS)
@@ -261,6 +276,7 @@ infl_k_members(const uint8_t *__restrict__ in, const InflMember *__restrict__ me
     }
     if (lane == 0) status[m] = st;
 }
+#endif
 
 // ---------------------------------------------------------------------------------------------------- host side
 inline const char *infl_status_text(int st) {

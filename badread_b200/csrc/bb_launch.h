@@ -70,3 +70,8 @@ void bbl_fasta_gather(cudaStream_t st, const uint8_t *src, const int64_t *src_lo
 // (index and offset) for input that is not BGZF or a corrupt member, as bb_bgzf_decompress; BB_ERR_CUDA otherwise.
 int bbl_bgzf_inflate_device(cudaStream_t st, const uint8_t *in, int64_t n, uint8_t **out, int64_t *total, char *msg,
                             size_t msg_len);
+// Any gzip stream in host memory in[0..n) inflated the same way (bb_tu_gunzip.cu): through bbl_bgzf_inflate_device when
+// every member is BGZF, else in chunks of chunk_bytes (0: the default); *stats as bb_gzip_decompress reports them.
+struct bb_gzip_stats;
+int bbl_gzip_inflate_device(cudaStream_t st, const uint8_t *in, int64_t n, int64_t chunk_bytes, uint8_t **out,
+                            int64_t *total, bb_gzip_stats *stats, char *msg, size_t msg_len);

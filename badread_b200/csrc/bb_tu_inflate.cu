@@ -13,6 +13,10 @@
 void bbm_set_error(const char *msg);   // bb_tu_models.cu
 int bbl_bgzf_inflate_device(cudaStream_t st, const uint8_t *in, int64_t n, uint8_t **out, int64_t *total, char *msg,
                             size_t msg_len);   // (bb_launch.h)
+int bbl_gzip_inflate_device(cudaStream_t st, const uint8_t *in, int64_t n, int64_t chunk_bytes, uint8_t **out,
+                            int64_t *total, bb_gzip_stats *stats, char *msg, size_t msg_len);   // (bb_launch.h)
+int bbl_gzip_chunked(cudaStream_t st, const uint8_t *in, int64_t n, int64_t chunk_bytes, uint8_t **out, int64_t *total,
+                     bb_gzip_stats *stats, char *msg, size_t msg_len);   // bb_tu_gunzip.cu
 
 namespace {
 
@@ -98,4 +102,21 @@ int bbl_bgzf_inflate_device(cudaStream_t st, const uint8_t *in, int64_t n, uint8
     std::vector<InflMember> members;
     if (!infl_walk(in, n, members, total, msg, msg_len)) return BB_ERR_ARG;
     return infl_device(st, in, n, members, *total, out, msg, msg_len);
+}
+
+// Any gzip stream: every member BGZF (the host walk succeeds) through infl_device, one warp per member; anything else
+// through the chunked inflater of bb_tu_gunzip.cu.  The choice is made from the input.
+int bbl_gzip_inflate_device(cudaStream_t st, const uint8_t *in, int64_t n, int64_t chunk_bytes, uint8_t **out,
+                            int64_t *total, bb_gzip_stats *stats, char *msg, size_t msg_len) {
+    *out = nullptr;
+    *total = 0;
+    *stats = bb_gzip_stats{};
+    std::vector<InflMember> members;
+    if (n > 0 && infl_walk(in, n, members, total, msg, msg_len)) {
+        stats->bgzf = 1;
+        stats->members = (int64_t)members.size();
+        return infl_device(st, in, n, members, *total, out, msg, msg_len);
+    }
+    *total = 0;
+    return bbl_gzip_chunked(st, in, n, chunk_bytes, out, total, stats, msg, msg_len);
 }

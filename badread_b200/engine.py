@@ -100,35 +100,16 @@ class FragmentBatch(object):
                 np.ascontiguousarray(lit), len(self.literals), np.asarray(self.target_identity, dtype=np.float64))
 
 
-def _is_bgzf(head):
-    """Whether a gzip member header carries the BC extra field of BGZF (SAM specification §4.1)."""
-    if len(head) < 18 or head[:3] != b'\x1f\x8b\x08' or not head[3] & 4:
-        return False
-    xlen = int.from_bytes(head[10:12], 'little')
-    f, end = 12, min(12 + xlen, len(head))
-    while f + 4 <= end:
-        if head[f:f + 2] == b'BC':
-            return True
-        f += 4 + int.from_bytes(head[f + 2:f + 4], 'little')
-    return False
-
-
 class FastaFile(object):
-    """The bytes of a FASTA file as Engine.load_fasta takes them, read once for all the engines: a plain or BGZF file as
-    it is, in page-locked memory (bb_host_alloc) so that it goes to the GPUs at the link's rate, with BGZF inflated on
-    the GPUs; a gzip file that is not BGZF is inflated here.  close() releases the memory."""
+    """The bytes of a FASTA file as Engine.load_fasta takes them, read once for all the engines: the file as it is, in
+    page-locked memory (bb_host_alloc) so that it goes to the GPUs at the link's rate.  A gzip file, BGZF or not, is
+    inflated on the GPUs.  close() releases the memory."""
 
     def __init__(self, filename):
         self._lib = _lib.lib()
         self._pinned = None
         with open(filename, 'rb') as f:
-            head = f.read(1 << 16)
-        self.bgzf = _is_bgzf(head)
-        if head[:2] == b'\x1f\x8b' and not self.bgzf:
-            import gzip
-            with gzip.open(filename, 'rb') as f:
-                self.data = np.frombuffer(f.read(), dtype=np.uint8)
-            return
+            self.gzip = f.read(2) == b'\x1f\x8b'
         size = os.path.getsize(filename)
         self._pinned, data = _host_alloc(max(size, 1))
         self.data = data[:size]
@@ -231,7 +212,7 @@ class Engine(object):
         try:
             n_hdr, n_text, n_kept = ctypes.c_int32(0), ctypes.c_int64(0), ctypes.c_int64(0)
             data = fasta.data
-            self._check(self._lib.bb_fasta_parse(self._ctx, _ptr(data) if data.size else None, data.size, int(fasta.bgzf),
+            self._check(self._lib.bb_fasta_parse(self._ctx, _ptr(data) if data.size else None, data.size, int(fasta.gzip),
                                                  ctypes.byref(n_hdr), ctypes.byref(n_text), ctypes.byref(n_kept)),
                         'bb_fasta_parse')
         finally:
@@ -251,6 +232,12 @@ class Engine(object):
         hi = np.asarray([r[1] for r in ranges] or [0], dtype=np.int64)
         self._check(self._lib.bb_fasta_reference(self._ctx, len(ranges), _ptr(lo), _ptr(hi)), 'bb_fasta_reference')
         return names, [b - a for a, b in ranges], depths, circular, hp_left, hp_right
+
+    def last_gzip_stats(self):
+        """How the last load_fasta inflated its file (bb_last_gzip_stats), as a dict: all zero for plain text."""
+        st = _lib.GzipStats()
+        self._check(self._lib.bb_last_gzip_stats(self._ctx, ctypes.byref(st)), 'bb_last_gzip_stats')
+        return st.as_dict()
 
     def download_reference(self, offset=0, n=None):
         """Bytes [offset, offset + n) of this GPU's reference (all from offset when n is None; the length is known to the

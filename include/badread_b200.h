@@ -85,12 +85,13 @@ BB_API const char *bb_version(void);
 BB_API int bb_upload_reference(bb_ctx *ctx, const uint8_t *bases, int64_t n_bases);
 
 /* The reference from a FASTA file parsed on the device, in place of bb_upload_reference: the bases never exist on the host.
- * bb_fasta_parse takes the file's bytes (page-locked memory copies fastest): the FASTA text itself, or with is_bgzf its
- * BGZF stream, inflated on the device as bb_bgzf_decompress inflates it (a gzip file that is not BGZF is inflated by the
- * caller).  It drops the context's reference, then parses with the semantics of misc.load_fasta_arrays: a line starting
+ * bb_fasta_parse takes the file's bytes (page-locked memory copies fastest): the FASTA text itself, or with is_bgzf (named
+ * for the BGZF files it first took) a gzip stream of it, BGZF or not, inflated on the device as bb_gzip_decompress
+ * inflates it.  It drops the context's reference, then parses with the semantics of misc.load_fasta_arrays: a line starting
  * with '>' is a header line; every other byte except '\n', '\r', ' ' and '\t' is kept, 'a'-'z' upper-cased.  It reports
- * the number of header lines, the bytes of their texts and the bytes kept; BB_ERR_ARG names a corrupt BGZF member (index
- * and offset) like bb_bgzf_decompress.  Device memory peaks at the input plus the text plus the kept bytes.
+ * the number of header lines, the bytes of their texts and the bytes kept; BB_ERR_ARG names a corrupt gzip member (index
+ * and offset) like bb_gzip_decompress, and bb_last_gzip_stats then tells how the stream was inflated.  Device memory peaks
+ * at the input plus the text plus the kept bytes, or at the inflater's peak (bb_gzip_decompress).
  * bb_fasta_headers then copies the header table: text[text_off[k] .. text_off[k + 1]) the text of header line k after
  * its '>' (without the newline, otherwise as in the file), kept_off[k] the bytes kept before it and kept_off[n] all of
  * them, so contig k's bases are kept bytes [kept_off[k], kept_off[k + 1]).  BB_ERR_CAPACITY if n_cap or text_cap is
@@ -100,6 +101,9 @@ BB_API int bb_upload_reference(bb_ctx *ctx, const uint8_t *bases, int64_t n_base
 BB_API int bb_fasta_parse(bb_ctx *ctx, const uint8_t *data, int64_t n, int is_bgzf, int32_t *n_headers, int64_t *text_bytes,
                           int64_t *n_kept);
 BB_API int bb_fasta_headers(bb_ctx *ctx, char *text, int64_t text_cap, int64_t *text_off, int64_t *kept_off, int32_t n_cap);
+/* How the last bb_fasta_parse inflated its gzip stream (all zero for plain text). */
+typedef struct bb_gzip_stats bb_gzip_stats;
+BB_API int bb_last_gzip_stats(const bb_ctx *ctx, bb_gzip_stats *stats);
 BB_API int bb_fasta_reference(bb_ctx *ctx, int32_t n_contigs, const int64_t *lo, const int64_t *hi);
 /* Copies bytes [offset, offset + n) of the context's reference to out (for checking what a load left on the device). */
 BB_API int bb_download_reference(bb_ctx *ctx, int64_t offset, int64_t n, uint8_t *out);
@@ -293,6 +297,32 @@ BB_API int bb_bam_compress(bb_ctx *ctx, const uint8_t *in, int64_t n, int64_t st
  *  Huffman table or code, a back-reference before its start, or does not match its CRC-32 or ISIZE; the message names the
  *  member (index and offset).  Malformed input never makes the kernel read or write outside the member. */
 BB_API int bb_bgzf_decompress(int device, const uint8_t *in, int64_t n, uint8_t *out, int64_t out_cap, int64_t *n_out);
+
+/* Inflates any gzip stream in[0..n) on `device`: one member or several, as gzip, pigz or zlib write them, with what
+ * Python's gzip.decompress accepts: NUL padding between and after members, FEXTRA, FNAME, FCOMMENT and FHCRC skipped
+ * (the header CRC is not checked).  Unlike Python it refuses a reserved header flag, as RFC 1952 asks.  A stream whose
+ * every member is BGZF goes through bb_bgzf_decompress's one warp per member; any other is cut into chunks of
+ * chunk_bytes compressed bytes (0: the default, 128 KiB) decoded side by side, each from a block start it finds itself,
+ * and stitched where one chunk's decoder stopped at the next one's start (csrc/bb_gunzip.cuh).  The choice is made from
+ * the input.  Every member's CRC-32 and ISIZE (mod 2^32) is checked.  Device memory peaks at about 11 bytes per input
+ * byte (the input and 16-bit symbol slots of 5 symbols per input byte) plus the output plus 32 KiB per chunk; more if
+ * a chunk inflates beyond 5 bytes per input byte, which makes every chunk decode again into larger slots.  The output size is known only once the stream has been inflated: *n_out = it, and BB_ERR_CAPACITY
+ * if out_cap is smaller (out may then be NULL), so that the caller asks again with the room.  BB_ERR_ARG for a corrupt
+ * stream, the message (bb_model_error()) naming the member by index and input offset.  stats (may be NULL) tells how the
+ * stream was inflated. */
+struct bb_gzip_stats {
+    int64_t members;          /* gzip members */
+    int64_t chunks;           /* chunks the deflate data were cut into (0 for BGZF) */
+    int64_t absorbed;         /* chunks without a block start, decoded as part of their predecessor */
+    int64_t first_candidate;  /* chunks after the first confirmed at the first block start they found */
+    int64_t repaired;         /* decodes of a chunk again from where its predecessor stopped, in repair launches */
+    int64_t chained;          /* ... and in the final serial chain */
+    int64_t reruns;           /* decodes run again with larger output slots */
+    int32_t bgzf;             /* 1: every member was BGZF (one warp per member) */
+    int32_t reserved;
+};
+BB_API int bb_gzip_decompress(int device, const uint8_t *in, int64_t n, uint8_t *out, int64_t out_cap, int64_t *n_out,
+                              int64_t chunk_bytes, bb_gzip_stats *stats);
 
 /* ---- host-side helpers (no GPU needed) -------------------------------------------------------------- */
 /* error_model.align_kmers (error_model.py:179-229) for a batch of (kmer, alt) pairs: kmers is n_alts*k bytes,
