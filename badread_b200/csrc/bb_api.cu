@@ -801,15 +801,15 @@ static int w_prepare(Worker &w) {
     BB_CUDA(&w, w.d_out_qual.ensure((size_t)w.out_cap + 16));
     // Lane pools of the window aligners and the leaf aligner.  Each alignment pipeline's leaf kernel owns half of the
     // history (checkpoints with lowmem), one lane per thread of its lane_ctas CTAs.  The window kernels run before the
-    // alignment and use the whole pool: the 4-word build up to 2 * lane_ctas CTAs, the 8-word build half as many (twice
-    // the words per lane), with lowmem both up to 2 * lane_ctas.
+    // alignment and use the whole pool: the 4-word build up to 2 * lane_ctas CTAs (band slices of up to 3 words per
+    // column), the 8-word build half as many (up to 7), with lowmem both up to 2 * lane_ctas.
     L.lane_ctas = c.sm_count * 4;
     const size_t lanes = (size_t)L.lane_ctas * 64;
     if (c.knobs.lowmem) {
         L.hist_per_pipe = lanes * BB_LEAF_MAX_TILES * BB_LEAF_CKPT_WORDS;
         BB_CUDA(&w, w.s_leafhist.ensure(2 * L.hist_per_pipe * sizeof(uint32_t)));
     } else {
-        L.hist_per_pipe = lanes * BB_LEAF_LANE_COLS * BB_LEAF_LW;  // per-column history
+        L.hist_per_pipe = lanes * BB_LEAF_LANE_COLS * (BB_LEAF_LW - 1);  // per-column band slices
         BB_CUDA(&w, w.s_lanehist.ensure(2 * L.hist_per_pipe * sizeof(uint2)));
     }
     BB_CUDA(&w, w.s_ltbuf.ensure(2 * lanes * BB_WIN_MAX_COLS));

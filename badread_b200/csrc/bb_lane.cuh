@@ -25,6 +25,9 @@ struct BBLaneProb {
 
 // Window words needed for a band: the window top is word max(0, (c - a) >> 5); rows up to c + b must fit.
 __device__ __forceinline__ int bb_lane_words(int a, int b) { return ((a + b) >> 5) + 2; }
+// Words of a band slice, the a + b + 1 rows c - a ... c + b of column c from row max(0, c - a) on: at most
+// bb_lane_words(a, b) - 1, so a window of LW words never needs more than LW - 1.
+__device__ __forceinline__ int bb_band_words(int a, int b) { return ((a + b) >> 5) + 1; }
 
 __device__ __forceinline__ void bb_lane_fetch(const BBLaneProb &P, int word, uint32_t &mA, uint32_t &mC, uint32_t &mG,
                                               uint32_t &mT) {
@@ -161,9 +164,10 @@ __device__ __forceinline__ void bb_prefetch_history(const uint2 *hist, int tj) {
 // columns down to tj - 2T + 1 that are not staged yet and waits only for the copies of the PREVIOUS tick.  A move goes at
 // most one column to the left, so the T columns a lane can reach before the next tick were requested one tick (T moves)
 // earlier and have arrived; the moves themselves read shared memory.  Slot of column c: c mod 2T (the columns a tick
-// overwrites are the ones the path has left behind).  Layout: ring[(slot * LW + word) * 64 + thread] (64 threads per
-// CTA: consecutive threads, consecutive 8-byte entries, no bank conflicts).
-#define BB_RING_BYTES(LW, T) (2 * (T) * (LW) * 64 * 8)
+// overwrites are the ones the path has left behind).  The history holds the band slice of every column (bw words at
+// hist[c * bw], bb_lane_step), at most LW - 1 words for a window of LW words.  Layout: ring[(slot * (LW - 1) + word) * 64
+// + thread] (64 threads per CTA: consecutive threads, consecutive 8-byte entries, no bank conflicts).
+#define BB_RING_BYTES(LW, T) (2 * (T) * ((LW) - 1) * 64 * 8)
 
 __device__ __forceinline__ void bb_cp_async8(uint2 *smem, const uint2 *gmem) {
 #if defined(__CUDA_ARCH__)
@@ -184,16 +188,18 @@ __device__ __forceinline__ void bb_cp_async_wait() {
 #endif
 }
 
-// One tick of a walking lane at column tj (>= 0).  staged_lo: lowest column requested so far; > tj marks a walk that
-// has not staged anything yet (it then issues two groups, so that the uniform wait below covers its first T columns).
-template <int LW, int T>
-__device__ __forceinline__ void bb_ring_tick(uint2 *ring, const uint2 *hist, int tj, int &staged_lo) {
+// One tick of a walking lane at column tj (>= 0) of a history of bw words per column; RW = LW - 1 words per ring slot.
+// staged_lo: lowest column requested so far; > tj marks a walk that has not staged anything yet (it then issues two
+// groups, so that the uniform wait below covers its first T columns).
+template <int RW, int T>
+__device__ __forceinline__ void bb_ring_tick(uint2 *ring, const uint2 *hist, int bw, int tj, int &staged_lo) {
     const bool fresh = staged_lo > tj;
     if (fresh) {
         const int lo1 = max(0, tj - T + 1);
         for (int col = tj; col >= lo1; col--) {
 #pragma unroll
-            for (int x = 0; x < LW; x++) bb_cp_async8(ring + ((col & (2 * T - 1)) * LW + x) * 64, hist + (long long)col * LW + x);
+            for (int x = 0; x < RW; x++)
+                if (x < bw) bb_cp_async8(ring + ((col & (2 * T - 1)) * RW + x) * 64, hist + (long long)col * bw + x);
         }
         bb_cp_async_commit();
         staged_lo = lo1;
@@ -201,24 +207,26 @@ __device__ __forceinline__ void bb_ring_tick(uint2 *ring, const uint2 *hist, int
     const int want_lo = max(0, tj - 2 * T + 1);
     for (int col = staged_lo - 1; col >= want_lo; col--) {
 #pragma unroll
-        for (int x = 0; x < LW; x++) bb_cp_async8(ring + ((col & (2 * T - 1)) * LW + x) * 64, hist + (long long)col * LW + x);
+        for (int x = 0; x < RW; x++)
+            if (x < bw) bb_cp_async8(ring + ((col & (2 * T - 1)) * RW + x) * 64, hist + (long long)col * bw + x);
     }
     bb_cp_async_commit();
     if (want_lo < staged_lo) staged_lo = want_lo;
 #if defined(__CUDA_ARCH__)
     // what the tick after the next one will ask for: into L2 now (HBM latency is more than one tick long)
     {
-        constexpr int LINES = (T * LW * 8 + 127) / 128 + 1;
-        const long long e = ((long long)tj - 4 * T) * LW;
+        constexpr int MAX_LINES = (T * RW * 8 + 127) / 128 + 1;
+        const int lines = (T * bw * 8 + 127) / 128 + 1;
+        const long long e = ((long long)tj - 4 * T) * bw;
 #pragma unroll
-        for (int x = 0; x < 2 * LINES; x++)
-            if (e + 16 * x >= 0 && (x < LINES || fresh)) asm volatile("prefetch.global.L2 [%0];" ::"l"(hist + e + 16 * x));
+        for (int x = 0; x < 2 * MAX_LINES; x++)
+            if (e + 16 * x >= 0 && x < (fresh ? 2 : 1) * lines) asm volatile("prefetch.global.L2 [%0];" ::"l"(hist + e + 16 * x));
     }
 #endif
     bb_cp_async_wait<1>();
 }
 
-template <int LW, int T>
+template <int RW, int T>
 __device__ __forceinline__ uint2 bb_ring_entry(const uint2 *ring, int col, int x) {
-    return ring[((col & (2 * T - 1)) * LW + x) * 64];
+    return ring[((col & (2 * T - 1)) * RW + x) * 64];
 }

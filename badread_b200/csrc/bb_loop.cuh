@@ -502,10 +502,11 @@ bb_k_window_lane(BBBatchDev B, BBErrorModelDev em, const BBWinTask *tasks, const
 }
 
 // The DEFAULT window aligner: one window alignment per thread; persistent lanes, all on the same step of the same phase;
-// per-column history (Pv, PhRaw per window word) in global memory.  The traceback does not chase it there: the columns
-// ahead of the path are staged in shared memory by cp.async, T columns per tick (bb_ring_tick), so a move costs a
-// shared-memory load instead of an L2 / HBM round trip.  The checkpoint build above (BADREAD_B200_LOWMEM=1) moves ~9 KB
-// per window instead of ~64 KB and is slower per step: recomputing tiles costs more than the traffic it saves.
+// per-column history (Pv, PhRaw of the band slice, bb_lane_step) in global memory.  The traceback does not chase it
+// there: the columns ahead of the path are staged in shared memory by cp.async, T columns per tick (bb_ring_tick), so a
+// move costs a shared-memory load instead of an L2 / HBM round trip.  The checkpoint build above (BADREAD_B200_LOWMEM=1)
+// moves ~9 KB per window instead of up to ~48 KB and is slower per step: recomputing tiles costs more than the traffic
+// it saves.
 #ifndef BB_WIN_RING_T
 #define BB_WIN_RING_T 4
 #endif
@@ -520,7 +521,7 @@ bb_k_window_lane_hist(BBBatchDev B, BBErrorModelDev em, const BBWinTask *tasks, 
 #endif
     const int n_tasks = *n_tasks_ptr;
     const long long gl = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    uint2 *const hist = hist_pool + gl * (long long)(BB_WIN_MAX_COLS * LW);
+    uint2 *const hist = hist_pool + gl * (long long)(BB_WIN_MAX_COLS * (LW - 1));
     uint8_t *const tbuf = tbuf_pool + gl * (long long)BB_WIN_MAX_COLS;
     uint2 *const ring = s_ring + threadIdx.x;
     BBLanePass<LW> S;
@@ -530,7 +531,7 @@ bb_k_window_lane_hist(BBBatchDev B, BBErrorModelDev em, const BBWinTask *tasks, 
     const uint32_t *state = nullptr;
     const unsigned int *ctime = nullptr;
     int phase = 0;  // 0: fetch, 1: join, 2: forward pass, 3: traceback, 4: done
-    int qpos = 0, qn = 0, jx = 0, tm = 0, uw = 0, ti = 0, tj = 0, diags = 0, dels = 0, dist = 0, staged_lo = 0;
+    int qpos = 0, qn = 0, jx = 0, tm = 0, uw = 0, ti = 0, tj = 0, diags = 0, dels = 0, dist = 0, staged_lo = 0, bw = 1;
     unsigned int tmax = 0;
     for (;;) {
         if (phase == 0) {
@@ -585,6 +586,7 @@ bb_k_window_lane_hist(BBBatchDev B, BBErrorModelDev em, const BBWinTask *tasks, 
                         P.n = qn; P.peq = B.fpeq + rd->fpeq_off; P.q = frag + qpos; P.qs = 1;
                         P.peq_bit0 = qpos + BB_PEQ_BIT0; P.t = tbuf; P.ts = 1;
                         bb_lane_begin<LW>(S, P);
+                        bw = bb_band_words(P.a, P.b);
                         phase = 2;
                     }
                 }
@@ -592,7 +594,7 @@ bb_k_window_lane_hist(BBBatchDev B, BBErrorModelDev em, const BBWinTask *tasks, 
         }
         for (int it = 0; it < 128; it++) {  // forward columns with history
             if (phase == 2) {
-                bb_lane_step<LW, true>(S, P, hist + (long long)S.c * LW);
+                bb_lane_step<LW, true>(S, P, hist + (long long)S.c * bw);
                 if (S.c >= tm) {
                     // '=' columns without looking at the characters again: the path's 'X' columns are the edit distance
                     // minus its 'I' and 'D' columns, and the diagonal moves are '=' or 'X'
@@ -605,13 +607,12 @@ bb_k_window_lane_hist(BBBatchDev B, BBErrorModelDev em, const BBWinTask *tasks, 
             if (phase == 3) {
                 if (ti >= 0 && tj >= 0) {
                     // (it is the same for all lanes: the walking lanes of the warp tick together)
-                    if ((it & (T - 1)) == 0) bb_ring_tick<LW, T>(ring, hist, tj, staged_lo);
-                    int wt = (tj - P.a) >> 5; if (wt < 0) wt = 0;
-                    const int x = (ti >> 5) - wt;
-                    if (x < 0 || x >= LW) { atomicOr(&B.reads[tk.r].flags, 1); ti = -1; tj = -1; }
+                    if ((it & (T - 1)) == 0) bb_ring_tick<LW - 1, T>(ring, hist, bw, tj, staged_lo);
+                    const int k = ti - max(0, tj - P.a);  // row in the band slice of column tj
+                    if (k < 0 || k >= 32 * bw) { atomicOr(&B.reads[tk.r].flags, 1); ti = -1; tj = -1; }
                     else {
-                        const uint2 e = bb_ring_entry<LW, T>(ring, tj, x);
-                        const int bit = ti & 31;
+                        const uint2 e = bb_ring_entry<LW - 1, T>(ring, tj, k >> 5);
+                        const int bit = k & 31;
                         if ((e.x >> bit) & 1u) ti--;
                         else if ((e.y >> bit) & 1u) { dels++; tj--; }
                         else { diags++; ti--; tj--; }

@@ -169,7 +169,8 @@ __device__ __forceinline__ void bb_lane_begin(BBLanePass<LW> &S, const BBProb &P
     S.wt = 0; S.score = 32 * LW; S.c = 0;
 }
 
-// One column of the pass. hist (optional): LW entries for this column, HSTRIDE apart.
+// One column of the pass. hist (optional): with HSTRIDE == 1, this column's band slice, the bb_band_words(a, b) words
+// from row max(0, c - a) on (the traceback never leaves the band); otherwise all LW window words, HSTRIDE apart.
 template <int LW, bool HIST, int HSTRIDE = 1>
 __device__ __forceinline__ void bb_lane_step(BBLanePass<LW> &S, const BBProb &P, uint2 *hist) {
     const int c = S.c;
@@ -217,13 +218,15 @@ __device__ __forceinline__ void bb_lane_step(BBLanePass<LW> &S, const BBProb &P,
         const uint32_t raw = Ph[x];
         S.Pv[x] = mhs | ~(Xv[x] | phs);
         S.Mv[x] = phs & Xv[x];
-        if (HIST && (HSTRIDE != 1 || (LW & 1))) hist[x * HSTRIDE] = make_uint2(S.Pv[x], raw);
-        if (HIST && HSTRIDE == 1 && !(LW & 1)) Ph[x] = raw;
+        if (HIST && HSTRIDE != 1) hist[x * HSTRIDE] = make_uint2(S.Pv[x], raw);
     }
-    if (HIST && HSTRIDE == 1 && !(LW & 1)) {  // a column's entries are contiguous and 16-byte aligned: 128-bit stores
+    if (HIST && HSTRIDE == 1) {
+        // the band's top row is bit off of window word 0 (wt = max(0, (c - a) >> 5)); Ph still holds the raw words
+        const int bw = bb_band_words(P.a, P.b);
+        const int off = c >= P.a ? (c - P.a) & 31 : 0;
 #pragma unroll
-        for (int x = 0; x < LW; x += 2)
-            reinterpret_cast<uint4 *>(hist)[x >> 1] = make_uint4(S.Pv[x], Ph[x], S.Pv[x + 1], Ph[x + 1]);
+        for (int y = 0; y + 1 < LW; y++)
+            if (y < bw) hist[y] = make_uint2(__funnelshift_r(S.Pv[y], S.Pv[y + 1], off), __funnelshift_r(Ph[y], Ph[y + 1], off));
     }
     S.c = c + 1;
 }
@@ -473,7 +476,7 @@ bb_k_leaf_lane_hist(BBBatchDev B, BBQueues Q, uint2 *hist_pool, int *cursor) {
 #endif
     const BBNode *list = Q.leaf[0];
     const int count = min(Q.count[BBQ_LEAF_COUNT], Q.cap_leaf);
-    uint2 *const hist = hist_pool + ((long long)blockIdx.x * blockDim.x + threadIdx.x) * (long long)(BB_LEAF_LANE_COLS * LW);
+    uint2 *const hist = hist_pool + ((long long)blockIdx.x * blockDim.x + threadIdx.x) * (long long)(BB_LEAF_LANE_COLS * (LW - 1));
     uint2 *const ring = s_ring + threadIdx.x;
     BBLanePass<LW> S;
     BBProb P;
@@ -501,7 +504,7 @@ bb_k_leaf_lane_hist(BBBatchDev B, BBQueues Q, uint2 *hist_pool, int *cursor) {
         if (__all_sync(BB_FULL, phase == 3)) break;
         for (int it = 0; it < 128; it++) {  // forward columns with history
             if (phase == 1) {
-                bb_lane_step<LW, true>(S, P, hist + (long long)S.c * LW);
+                bb_lane_step<LW, true>(S, P, hist + (long long)S.c * bb_band_words(P.a, P.b));
                 if (S.c >= nd.mm) {
                     const int d = bb_lane_corner<LW>(S, nd.nn);
                     if (nd.best >= 0 && d != nd.best) atomicOr(&o.rd->flags, 8 << 8);
@@ -514,13 +517,13 @@ bb_k_leaf_lane_hist(BBBatchDev B, BBQueues Q, uint2 *hist_pool, int *cursor) {
             if (phase == 2) {
                 if (ti >= 0 && tj >= 0) {
                     // (it is the same for all lanes: the walking lanes of the warp tick together)
-                    if ((it & (T - 1)) == 0) bb_ring_tick<LW, T>(ring, hist, tj, staged_lo);
-                    int wt = (tj - P.a) >> 5; if (wt < 0) wt = 0;
-                    const int x = (ti >> 5) - wt;
-                    if (x < 0 || x >= LW) { atomicOr(&o.rd->flags, 1 << 8); ti = -1; tj = -1; }
+                    const int bw = bb_band_words(P.a, P.b);  // (recomputed, not kept: a live register more spills)
+                    if ((it & (T - 1)) == 0) bb_ring_tick<LW - 1, T>(ring, hist, bw, tj, staged_lo);
+                    const int k = ti - max(0, tj - P.a);  // row in the band slice of column tj
+                    if (k < 0 || k >= 32 * bw) { atomicOr(&o.rd->flags, 1 << 8); ti = -1; tj = -1; }
                     else {
-                        const uint2 e = bb_ring_entry<LW, T>(ring, tj, x);
-                        const int bit = ti & 31;
+                        const uint2 e = bb_ring_entry<LW - 1, T>(ring, tj, k >> 5);
+                        const int bit = k & 31;
                         if ((e.x >> bit) & 1u) { o.ops[nd.q0 + ti] = BB_OP_I; ti--; }
                         else if ((e.y >> bit) & 1u) { bb_add_dels(o, nd.q0 + ti, 1); dels++; tj--; }
                         else {

@@ -1,8 +1,8 @@
 // bb_tu_window_hist.cu — compiles the default lane-mode window aligners bb_k_window_lane_hist<4>, <8> (bb_loop.cuh).
 #include "bb_launch.h"
 
-// ring_t: columns staged per traceback tick (bb_ring_tick); 8 halves the ticks of the 4-word build at 7 instead of 8
-// CTAs per SM (32 KB of shared memory per CTA)
+// ring_t: columns staged per traceback tick (bb_ring_tick); 8 halves the ticks of the 4-word build (24 KB of shared
+// memory per CTA)
 void bbl_window_lane_hist(int words, int ring_t, int grid, cudaStream_t st, BBBatchDev B, BBErrorModelDev em,
                           const BBWinTask *tasks, const int *n_tasks, unsigned long long seed, uint2 *hist_pool,
                           uint8_t *tbuf_pool, int *cursor, BBWinTask *fallback, int *fallback_count) {
