@@ -88,6 +88,15 @@ class AlnView(ctypes.Structure):
                                         'cigar', 'cigar_off', 'seq', 'qual', 'seq_off', 'has_qual', 'full')]
 
 
+class FlatView(ctypes.Structure):
+    """bb_flat_view (include/badread_b200.h)."""
+    _fields_ = [('n', ctypes.c_int32)] + [(f, ctypes.c_void_p) for f in ('read', 'qual', 'ref', 'ops', 'op_read0', 'op_ref0',
+                                                                           'read_off', 'ref_off', 'ops_off')]
+
+
+BB_ALN_PAF = 2
+
+
 class LibraryMissing(RuntimeError):
     pass
 
@@ -173,6 +182,13 @@ def lib():
         'bb_aln_parse': (c.c_int, [vp, i64, c.c_int, i64, P(vp)]),
         'bb_aln_view_get': (c.c_int, [vp, P(AlnView)]),
         'bb_aln_free': (c.c_int, [vp]),
+        'bb_device_count': (c.c_int, []),
+        'bb_fastq_parse': (c.c_int, [c.c_int, vp, i64, c.c_int, P(vp), P(i64), P(i32)]),
+        'bb_fastq_free': (c.c_int, [vp]),
+        'bb_flat_build': (c.c_int, [vp, P(AlnView), i32, vp, vp, vp, vp, i64, P(vp), vp]),
+        'bb_flat_view_get': (c.c_int, [vp, P(FlatView)]),
+        'bb_flat_fetch': (c.c_int, [vp, c.c_int, i64, i64, vp]),
+        'bb_flat_free': (c.c_int, [vp]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(L, name)
@@ -194,4 +210,5 @@ EXPORTED_SYMBOLS = ['bb_create', 'bb_destroy', 'bb_last_error', 'bb_version', 'b
                     'bb_bgzf_bound', 'bb_bgzf_compress', 'bb_bgzf_decompress', 'bb_aln_parse', 'bb_aln_view_get', 'bb_aln_free',
                     'bb_fetch_last_batch_results', 'bb_bam_build', 'bb_bam_compress_device', 'bb_bam_fetch_records',
                     'bb_bam_compress', 'bb_bam_layout_sharded', 'bb_fasta_parse', 'bb_fasta_headers', 'bb_fasta_reference',
-                    'bb_download_reference', 'bb_gzip_decompress', 'bb_last_gzip_stats']
+                    'bb_download_reference', 'bb_gzip_decompress', 'bb_last_gzip_stats', 'bb_device_count', 'bb_fastq_parse',
+                    'bb_fastq_free', 'bb_flat_build', 'bb_flat_view_get', 'bb_flat_fetch', 'bb_flat_free']

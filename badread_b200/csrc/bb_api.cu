@@ -314,6 +314,14 @@ static int each_worker(bb_ctx *ctx, F &&f) {
     return BB_OK;
 }
 
+// misc.REV_COMP_DICT (misc.py:56-61); anything else complements to 'N' (misc.py:64-68)
+void bbl_comp_table(uint8_t *table) {
+    std::memset(table, 'N', 256);
+    const char *from = "ATGCatgcRYSWKMBVDHNryswkmbvdhn.-?";
+    const char *to = "TACGtacgYRSWMKVBHDNyrswmkvbhdn.-?";
+    for (int i = 0; from[i]; i++) table[(uint8_t)from[i]] = (uint8_t)to[i];
+}
+
 extern "C" const char *bb_version(void) { return "badread_b200 0.1.0 (sm_90a)"; }
 
 extern "C" const char *bb_last_error(const bb_ctx *ctx) { return ctx ? ctx->err.c_str() : g_create_error.c_str(); }
@@ -373,12 +381,8 @@ extern "C" int bb_create(bb_ctx **out, int device, uint64_t seed) {
     ctx->sm_count = prop.multiProcessorCount;
     // persistent warps: 4 CTAs of 4 warps per SM for the warp-per-read kernels
     ctx->n_warps = ctx->sm_count * 4 * BB_WARPS_PER_CTA;
-    // misc.REV_COMP_DICT (misc.py:56-61); anything else complements to 'N' (misc.py:64-68)
     uint8_t comp[256];
-    std::memset(comp, 'N', sizeof(comp));
-    const char *from = "ATGCatgcRYSWKMBVDHNryswkmbvdhn.-?";
-    const char *to = "TACGtacgYRSWMKVBHDNyrswmkvbhdn.-?";
-    for (int i = 0; from[i]; i++) comp[(uint8_t)from[i]] = (uint8_t)to[i];
+    bbl_comp_table(comp);
     e = cudaMemcpyToSymbol(bb_c_comp, comp, 256);
     if (e == cudaSuccess) e = bbl_node_pair_init();
     if (e == cudaSuccess) e = bbl_node_quad_init();

@@ -1,4 +1,4 @@
-// bb_bam.cpp — SAM and BAM alignment records for the model builders (include/badread_b200.h, bb_aln_parse): the fields
+// bb_bam.cpp — SAM, BAM and PAF alignment records for the model builders (include/badread_b200.h, bb_aln_parse): the fields
 // of the PAF line the reference's builders would read, per mapped record, from the CIGAR, POS, FLAG and the AS:i / NM:i
 // tags, plus SEQ and QUAL.  BAM arrives already inflated (bb_bgzf_decompress); records may have straddled BGZF members,
 // which no longer matters here.  Host code: one pass over the records, no per-record work left to the caller.
@@ -282,6 +282,105 @@ void parse_bam(bb_aln_set &S, const uint8_t *d, int64_t n, int64_t max_records) 
     }
 }
 
+// str.strip()'s ASCII whitespace
+bool paf_space(char c) { return c == ' ' || (c >= '\t' && c <= '\r') || (c >= 0x1c && c <= 0x1f); }
+
+// PAF text as model_builders.Alignment reads it, line by line (text mode: '\n', "\r\n" and a lone '\r' end lines)
+void parse_paf(bb_aln_set &S, const char *text, int64_t n, int64_t max_records) {
+    int64_t line_no = 0;
+    std::vector<std::pair<const char *, const char *>> f;
+    for (const char *p = text, *end = text + n; p < end;) {
+        const char *q = p;
+        while (q < end && *q != '\n' && *q != '\r') q++;
+        const char *line = p, *le = q;
+        p = q == end ? end : (*q == '\r' && q + 1 < end && q[1] == '\n') ? q + 2 : q + 1;
+        line_no++;
+        while (line < le && paf_space(*line)) line++;
+        while (le > line && paf_space(le[-1])) le--;
+        f.clear();
+        for (const char *c = line;;) {
+            const char *tab = (const char *)std::memchr(c, '\t', (size_t)(le - c));
+            f.emplace_back(c, tab ? tab : le);
+            if (!tab) break;
+            c = tab + 1;
+        }
+        if (f.size() < 11) throw Fail{"Error: alignment file does not seem to be in PAF format"};
+        // int() of a field: surrounding whitespace, an optional sign, decimal digits
+        auto num = [&](const char *a, const char *b, int64_t lo, int64_t hi, const char *what) {
+            while (a < b && paf_space(*a)) a++;
+            while (b > a && paf_space(b[-1])) b--;
+            int64_t v = 0;
+            if (!parse_int(a, b, &v) || v < lo || v > hi) {
+                char msg[160];
+                std::snprintf(msg, sizeof(msg), "Error: %s on line %lld of the alignment file is not an integer in [%lld, %lld]",
+                              what, (long long)line_no, (long long)lo, (long long)hi);
+                throw Fail{msg};
+            }
+            return v;
+        };
+        auto col = [&](int k, int64_t lo, int64_t hi) {
+            static const char *names[] = {"", "", "column 3", "column 4", "", "", "", "column 8", "column 9", "column 10", "column 11"};
+            return num(f[k].first, f[k].second, lo, hi, names[k]);
+        };
+        const int64_t qs = col(2, INT32_MIN, INT32_MAX), qe = col(3, INT32_MIN, INT32_MAX);
+        const int64_t ts = col(7, -((int64_t)1 << 40), (int64_t)1 << 40), te = col(8, -((int64_t)1 << 40), (int64_t)1 << 40);
+        const int64_t matching = col(9, INT32_MIN, INT32_MAX), cols = col(10, INT32_MIN, INT32_MAX);
+        if (cols == 0) {
+            char msg[128];
+            std::snprintf(msg, sizeof(msg), "Error: line %lld of the alignment file has 0 alignment columns (column 11)", (long long)line_no);
+            throw Fail{msg};
+        }
+        if (cols - matching < INT32_MIN || cols - matching > INT32_MAX) {
+            char msg[128];
+            std::snprintf(msg, sizeof(msg), "Error: columns 10 and 11 on line %lld of the alignment file are out of range", (long long)line_no);
+            throw Fail{msg};
+        }
+        const char *cg = nullptr, *cg_end = nullptr;
+        bool has_as = false;
+        int64_t as = 0;
+        for (auto &x : f) {   // every column, the last tag of each kind wins
+            if (x.second - x.first >= 5 && std::memcmp(x.first, "cg:Z:", 5) == 0) { cg = x.first + 5; cg_end = x.second; }
+            if (x.second - x.first >= 5 && std::memcmp(x.first, "AS:i:", 5) == 0) {
+                as = num(x.first + 5, x.second, INT32_MIN, INT32_MAX, "the AS:i: tag");
+                has_as = true;
+            }
+        }
+        if (!cg) throw Fail{"Error: no CIGAR string found"};
+        if (!has_as) throw Fail{"Error: no alignment score"};
+        const std::string name(f[0].first, f[0].second);
+        for (const char *c = cg; c < cg_end;) {   // re.findall(r'(\d+)([A-Za-z=])')
+            if (*c < '0' || *c > '9') { c++; continue; }
+            const char *d = c;
+            while (d < cg_end && *d >= '0' && *d <= '9') d++;
+            const bool letter = d < cg_end && ((*d >= 'A' && *d <= 'Z') || (*d >= 'a' && *d <= 'z') || *d == '=');
+            if (!letter) { c = d; continue; }
+            const uint32_t code = *d == 'M' ? OP_M : *d == 'I' ? OP_I : *d == 'D' ? OP_D : 15u;
+            int64_t len = 0;
+            for (const char *x = c; x < d && len < ((int64_t)1 << 28); x++) len = len * 10 + (*x - '0');
+            if (code != 15u && len >= ((int64_t)1 << 28)) throw Fail{"Error: a CIGAR run of read " + name + " is longer than 2^28 - 1"};
+            S.cigar.push_back(((uint32_t)(code == 15u ? 0 : len) << 4) | code);
+            c = d + 1;
+        }
+        const bool reverse = f[4].second - f[4].first == 1 && *f[4].first == '-';
+        S.read_id.push_back(S.read(name.data(), name.size()));
+        S.ref_id.push_back(S.ref(f[5].first, (size_t)(f[5].second - f[5].first)));
+        S.flag.push_back(reverse ? 16 : 0);
+        S.score.push_back((int32_t)as);
+        S.nm.push_back((int32_t)(cols - matching));
+        S.read_len.push_back(0);
+        S.read_start.push_back((int32_t)qs);
+        S.read_end.push_back((int32_t)qe);
+        S.columns.push_back((int32_t)cols);
+        S.ref_start.push_back(ts);
+        S.ref_end.push_back(te);
+        S.cigar_off.push_back((int64_t)S.cigar.size());
+        S.has_qual.push_back(0);
+        S.full.push_back(0);
+        S.seq_off.push_back((int64_t)S.seq.size());
+        if (line_no == max_records) break;
+    }
+}
+
 }  // namespace
 
 extern "C" int bb_aln_parse(const uint8_t *data, int64_t n, int is_bam, int64_t max_records, bb_aln_set **set) {
@@ -293,7 +392,8 @@ extern "C" int bb_aln_parse(const uint8_t *data, int64_t n, int is_bam, int64_t 
     *set = nullptr;
     bb_aln_set *S = new bb_aln_set();
     try {
-        if (is_bam) parse_bam(*S, data, n, max_records);
+        if (is_bam == BB_ALN_PAF) parse_paf(*S, (const char *)data, n, max_records);
+        else if (is_bam) parse_bam(*S, data, n, max_records);
         else parse_sam(*S, (const char *)data, n, max_records);
     } catch (const Fail &f) {
         bbm_set_error(f.msg.c_str());

@@ -62,6 +62,8 @@ void bbl_fasta_scan(cudaStream_t st, const uint8_t *text, int64_t n, void *scrat
 const int64_t *bbl_fasta_totals(const void *scratch, int64_t n);
 void bbl_fasta_emit(cudaStream_t st, const uint8_t *text, int64_t n, const void *scratch, uint8_t *kept, int64_t *hdr_start,
                     int64_t *hdr_end, int64_t *hdr_kept);
+// bb_c_comp's table (misc._COMP_TABLE) into table[256], for every unit that complements on the device
+void bbl_comp_table(uint8_t *table);
 // dst[dst_off[r] .. dst_off[r + 1]) = src[src_lo[r] ..] for r < n_ranges; total = dst_off[n_ranges] (device arrays)
 void bbl_fasta_gather(cudaStream_t st, const uint8_t *src, const int64_t *src_lo, const int64_t *dst_off, int32_t n_ranges,
                       int64_t total, uint8_t *dst);

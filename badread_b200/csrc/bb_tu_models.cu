@@ -36,6 +36,17 @@ struct DevMem {   // everything a call allocates, released on every exit path
         else if (fill >= 0) e = cudaMemset(q, fill, bytes ? bytes : 16);
         return e;
     }
+    // an input array: used in place when it is device memory of `device`, else copied like get()
+    template <typename X>
+    cudaError_t input(X **out, size_t bytes, const X *src, int device) {
+        cudaPointerAttributes at{};
+        if (cudaPointerGetAttributes(&at, src) == cudaSuccess && at.type == cudaMemoryTypeDevice && at.device == device) {
+            *out = const_cast<X *>(src);
+            return cudaSuccess;
+        }
+        (void)cudaGetLastError();
+        return get(out, bytes, src);
+    }
 };
 
 #define BBM_TRY(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { \
@@ -70,15 +81,15 @@ int count_common(bool qscores, bool wide, int device, int k, int max_del, int32_
     int64_t *d_read_off, *d_ref_off, *d_ops_off;
     uint32_t *d_ops;
     int32_t *d_p0, *d_r0;
-    BBM_TRY(mem.get(&d_read, (size_t)n_read, read));
-    if (qscores) BBM_TRY(mem.get(&d_qual, (size_t)n_read, qual));
-    BBM_TRY(mem.get(&d_ref, (size_t)n_ref, ref));
+    BBM_TRY(mem.input(&d_read, (size_t)n_read, read, device));
+    if (qscores) BBM_TRY(mem.input(&d_qual, (size_t)n_read, qual, device));
+    BBM_TRY(mem.input(&d_ref, (size_t)n_ref, ref, device));
     BBM_TRY(mem.get(&d_read_off, (size_t)(n_aln + 1) * 8, read_off));
     BBM_TRY(mem.get(&d_ref_off, (size_t)(n_aln + 1) * 8, ref_off));
     BBM_TRY(mem.get(&d_ops_off, (size_t)(n_aln + 1) * 8, ops_off));
-    BBM_TRY(mem.get(&d_ops, (size_t)n_ops * 4, ops));
-    BBM_TRY(mem.get(&d_p0, (size_t)n_ops * 4, op_read0));
-    BBM_TRY(mem.get(&d_r0, (size_t)n_ops * 4, op_ref0));
+    BBM_TRY(mem.input(&d_ops, (size_t)n_ops * 4, ops, device));
+    BBM_TRY(mem.input(&d_p0, (size_t)n_ops * 4, op_read0, device));
+    BBM_TRY(mem.input(&d_r0, (size_t)n_ops * 4, op_ref0, device));
     A.read = d_read; A.qual = d_qual; A.ref = d_ref; A.read_off = d_read_off; A.ref_off = d_ref_off; A.ops_off = d_ops_off;
     A.ops = d_ops; A.op_read0 = d_p0; A.op_ref0 = d_r0;
     BBMTable T{};

@@ -13,6 +13,10 @@ The alignments may also be SAM (plain or gzipped) or BAM, told apart from PAF by
 BAM's BGZF members are inflated on the GPU (bgzf.decompress); native host code (csrc/bb_bam.cpp) turns the records of
 either into the fields of the PAF line the reference would read, and the best alignment per read is chosen here with
 the rules of load_alignments, over arrays.  Without --reads the sequences and qualities come from the records.
+
+With PAF alignments, --reads and a CUDA device (device_route) the FASTQ is parsed on the GPU, the PAF by bb_aln_parse and
+the aligned slices are gathered on the GPU into a DeviceFlat (csrc/bb_tu_fastq.cu), which the counting kernels read in
+place; the same messages, progress text and model files as the host route above.
 """
 import collections
 import ctypes
@@ -23,7 +27,7 @@ import sys
 import numpy as np
 
 from . import _lib, bgzf
-from .misc import float_to_str, get_open_func, load_fasta, reverse_complement
+from .misc import float_to_str, get_compression_type, get_open_func, load_fasta, reverse_complement
 
 _CIGAR_RUN = re.compile(r'(\d+)([A-Za-z=])')
 _OP_CODE = {'M': 0, 'I': 1, 'D': 2}
@@ -165,6 +169,60 @@ def _names(blob_ptr, off):
     return [blob[a:b].decode() for a, b in zip(off[:-1].tolist(), off[1:].tolist())]
 
 
+def _parse_records(filename, fmt, max_alignments):
+    """bb_aln_parse of a SAM, BAM or PAF file (a BAM's BGZF and a gzipped PAF inflated on the GPU): its handle (bb_aln_free
+    it)."""
+    with (open if fmt in ('bam', 'paf') else get_open_func(filename))(filename, 'rb') as handle:
+        data = handle.read()
+    if fmt == 'bam':
+        try:
+            data = _inflate(data)
+        except ValueError as e:
+            sys.exit(f'\nError: {filename} is not a valid BAM file ({e})')
+    elif fmt == 'paf' and get_compression_type(filename) == 'gz':
+        try:
+            data = bgzf.gunzip(data)[0]
+        except ValueError as e:
+            sys.exit(f'\nError: {filename} could not be inflated ({e})')
+    L = _lib.lib()
+    buf = np.frombuffer(memoryview(data).cast('B'), dtype=np.uint8)
+    handle = ctypes.c_void_p()
+    rc = L.bb_aln_parse(buf.ctypes.data_as(ctypes.c_void_p) if buf.size else None, buf.size,
+                        {'sam': 0, 'bam': 1, 'paf': _lib.BB_ALN_PAF}[fmt], max_alignments or 0, ctypes.byref(handle))
+    if rc != _lib.BB_OK:      # (load_alignments' messages end its unfinished line; bb_aln_parse's SAM / BAM ones break it)
+        sys.exit(('' if fmt == 'paf' else '\n') + L.bb_model_error().decode(errors='replace'))
+    return handle
+
+
+def _record_arrays(handle):
+    """(bb_aln_view, records, reference names, read names, {field: array}) of a bb_aln_parse handle."""
+    v = _lib.AlnView()
+    _lib.lib().bb_aln_view_get(handle, ctypes.byref(v))
+    n = v.n_records
+    ref_names = _names(v.ref_names, _view_array(v.ref_name_off, v.n_refs + 1, np.int64))
+    read_names = _names(v.read_names, _view_array(v.read_name_off, v.n_reads + 1, np.int64))
+    a = {f: _view_array(getattr(v, f), n, t) for f, t in
+         (('read_id', np.int32), ('ref_id', np.int32), ('flag', np.int32), ('score', np.int32), ('nm', np.int32),
+          ('read_start', np.int32), ('read_end', np.int32), ('columns', np.int32), ('ref_start', np.int64),
+          ('ref_end', np.int64), ('has_qual', np.uint8), ('full', np.uint8))}
+    return v, n, ref_names, read_names, a
+
+
+def _best_per_read(a, n):
+    """Per read the record with the highest score, the last among equals; reads in order of first appearance."""
+    order = np.lexsort((np.arange(n), a['score'], a['read_id']))           # per read: by score, then by position
+    last = np.flatnonzero(np.append(a['read_id'][order][1:] != a['read_id'][order][:-1], True)) if n else order
+    return order[last]
+
+
+def _usable(best, columns, matches):
+    """The records of `best` with more than 100 columns and more than 80 % identity (Alignment.percent_identity's two
+    operations)."""
+    cols = columns.astype(np.int64)
+    with np.errstate(divide='ignore', invalid='ignore'):
+        return best[(cols > 100) & (100.0 * matches / cols > 80.0)]
+
+
 def load_sam_alignments(filename, fmt, max_alignments, reads, refs, need_qual, output=sys.stderr, dot_interval=1000):
     """The alignments of a SAM or BAM file, chosen as load_alignments chooses them: per read the record with the highest
     AS:i (the last among equals), kept with more than 100 columns and more than 80 % identity, reads in order of first
@@ -173,30 +231,10 @@ def load_sam_alignments(filename, fmt, max_alignments, reads, refs, need_qual, o
     every chosen read's sequence and qualities from a record of it that holds the whole read (SEQ not '*', no H clip),
     turned back to the read's own orientation.  Returns (alignments, reads)."""
     print('Loading alignments', end='', file=output, flush=True)
-    with (open if fmt == 'bam' else get_open_func(filename))(filename, 'rb') as handle:
-        data = handle.read()
-    if fmt == 'bam':
-        try:
-            data = _inflate(data)
-        except ValueError as e:
-            sys.exit(f'\nError: {filename} is not a valid BAM file ({e})')
     L = _lib.lib()
-    buf = np.frombuffer(memoryview(data).cast('B'), dtype=np.uint8)
-    handle = ctypes.c_void_p()
-    rc = L.bb_aln_parse(buf.ctypes.data_as(ctypes.c_void_p) if buf.size else None, buf.size, int(fmt == 'bam'),
-                        max_alignments or 0, ctypes.byref(handle))
-    if rc != _lib.BB_OK:
-        sys.exit('\n' + L.bb_model_error().decode(errors='replace'))
+    handle = _parse_records(filename, fmt, max_alignments)
     try:
-        v = _lib.AlnView()
-        L.bb_aln_view_get(handle, ctypes.byref(v))
-        n = v.n_records
-        ref_names = _names(v.ref_names, _view_array(v.ref_name_off, v.n_refs + 1, np.int64))
-        read_names = _names(v.read_names, _view_array(v.read_name_off, v.n_reads + 1, np.int64))
-        a = {f: _view_array(getattr(v, f), n, t) for f, t in
-             (('read_id', np.int32), ('ref_id', np.int32), ('flag', np.int32), ('score', np.int32), ('nm', np.int32),
-              ('read_start', np.int32), ('read_end', np.int32), ('columns', np.int32), ('ref_start', np.int64),
-              ('ref_end', np.int64), ('has_qual', np.uint8), ('full', np.uint8))}
+        v, n, ref_names, read_names, a = _record_arrays(handle)
         cigar_off = _view_array(v.cigar_off, n + 1, np.int64)
         cigar = _view_array(v.cigar, int(cigar_off[-1]), np.uint32)
         seq_off = _view_array(v.seq_off, n + 1, np.int64)
@@ -207,9 +245,7 @@ def load_sam_alignments(filename, fmt, max_alignments, reads, refs, need_qual, o
     print('.' * (n // dot_interval), file=output, flush=True)
 
     print('Choosing best alignment per read', end='', file=output, flush=True)
-    order = np.lexsort((np.arange(n), a['score'], a['read_id']))           # per read: by score, then by position
-    last = np.flatnonzero(np.append(a['read_id'][order][1:] != a['read_id'][order][:-1], True)) if n else order
-    best = order[last]                                                      # reads in order of first appearance
+    best = _best_per_read(a, n)
 
     def whole_read(i):
         """The read of record i's own orientation from the record of it that holds the whole read."""
@@ -237,9 +273,7 @@ def load_sam_alignments(filename, fmt, max_alignments, reads, refs, need_qual, o
     for k in np.flatnonzero(a['nm'][best] < 0).tolist():                    # no NM:i: count from the sequences
         i = int(best[k])
         matches[k] = _count_matches(i, a, cigar, cigar_off, whole_read(i), refs.get(ref_names[a['ref_id'][i]]))
-    cols = a['columns'][best].astype(np.int64)
-    with np.errstate(divide='ignore', invalid='ignore'):
-        keep = best[(cols > 100) & (100.0 * matches / cols > 80.0)]
+    keep = _usable(best, a['columns'][best], matches)
     chosen = []
     for i in keep.tolist():
         name = read_names[a['read_id'][i]]
@@ -343,27 +377,217 @@ class FlatAlignments(object):
         """Per read base of alignment a: symbol and the number of 'D' columns behind it; per reference base: the read
         offset at its column and whether that column holds a read base."""
         lo, hi = int(self.ops_off[a]), int(self.ops_off[a + 1])
-        read = self.read[self.read_off[a]:self.read_off[a + 1]]
-        ref = self.ref[self.ref_off[a]:self.ref_off[a + 1]]
-        sym = np.zeros(len(read), dtype=np.uint8)
-        dcount = np.zeros(len(read), dtype=np.int64)
-        rp_at = np.zeros(len(ref), dtype=np.int64)
-        is_m = np.zeros(len(ref), dtype=bool)
-        lead = 0
-        for o in range(lo, hi):
-            count, kind, p, r = int(self.ops[o]) >> 2, int(self.ops[o]) & 3, int(self.op_read0[o]), int(self.op_ref0[o])
-            if kind == 0:
-                sym[p:p + count] = (read[p:p + count] != ref[r:r + count]).astype(np.uint8)
-                rp_at[r:r + count] = np.arange(p, p + count); is_m[r:r + count] = True
-            elif kind == 1:
-                sym[p:p + count] = 2
+        return _columns(self.read[self.read_off[a]:self.read_off[a + 1]], self.ref[self.ref_off[a]:self.ref_off[a + 1]],
+                        self.ops[lo:hi], self.op_read0[lo:hi], self.op_ref0[lo:hi])
+
+    def quals(self, a):
+        """The quality slice of alignment a."""
+        return self.qual[self.read_off[a]:self.read_off[a + 1]]
+
+
+def _columns(read, ref, ops, op_read0, op_ref0):
+    """FlatAlignments.columns of one alignment's slices and runs."""
+    sym = np.zeros(len(read), dtype=np.uint8)
+    dcount = np.zeros(len(read), dtype=np.int64)
+    rp_at = np.zeros(len(ref), dtype=np.int64)
+    is_m = np.zeros(len(ref), dtype=bool)
+    lead = 0
+    for o in range(len(ops)):
+        count, kind, p, r = int(ops[o]) >> 2, int(ops[o]) & 3, int(op_read0[o]), int(op_ref0[o])
+        if kind == 0:
+            sym[p:p + count] = (read[p:p + count] != ref[r:r + count]).astype(np.uint8)
+            rp_at[r:r + count] = np.arange(p, p + count); is_m[r:r + count] = True
+        elif kind == 1:
+            sym[p:p + count] = 2
+        else:
+            rp_at[r:r + count] = p
+            if p > 0:
+                dcount[p - 1] += count
             else:
-                rp_at[r:r + count] = p
-                if p > 0:
-                    dcount[p - 1] += count
-                else:
-                    lead += count
-        return read, ref, sym, dcount, rp_at, is_m, lead
+                lead += count
+    return read, ref, sym, dcount, rp_at, is_m, lead
+
+
+# ---------------------------------------------------------------------------------------------------- device route
+def device_route(args, fmt):
+    """The route hook: True when a builder takes the device route - PAF alignments with --reads, and the library sees a
+    CUDA device.  The FASTQ is then parsed on the GPU and the aligned slices gathered there (csrc/bb_tu_fastq.cu), the
+    PAF parsed by native code (bb_aln_parse), and the counting kernels take the flat arrays where they lie (DeviceFlat).
+    Otherwise the host route: load_fastq, load_alignments / load_sam_alignments and FlatAlignments."""
+    if fmt != 'paf' or args.reads is None:
+        return False
+    try:
+        return _lib.lib().bb_device_count() > 0
+    except (_lib.LibraryMissing, OSError):
+        return False
+
+
+class DeviceFlat(object):
+    """FlatAlignments in device memory (bb_flat_build): the same attributes and dtypes, the offsets on the host and the
+    other arrays copied to the host on first access; columns(a) fetches alignment a's slices only; device_pointers are
+    what _count passes to the counting kernels.  close() releases the device memory."""
+    _ARRAYS = {'read': (0, np.uint8, 'read_off'), 'qual': (1, np.uint8, 'read_off'), 'ref': (2, np.uint8, 'ref_off'),
+               'ops': (3, np.uint32, 'ops_off'), 'op_read0': (4, np.int32, 'ops_off'), 'op_ref0': (5, np.int32, 'ops_off')}
+
+    def __init__(self, handle):
+        self._handle = handle
+        v = _lib.FlatView()
+        _lib.lib().bb_flat_view_get(handle, ctypes.byref(v))
+        self.n = v.n
+        self.read_off = _view_array(v.read_off, self.n + 1, np.int64)
+        self.ref_off = _view_array(v.ref_off, self.n + 1, np.int64)
+        self.ops_off = _view_array(v.ops_off, self.n + 1, np.int64)
+        self.device_pointers = [ctypes.c_void_p(getattr(v, f)) for f in ('read', 'qual', 'ref', 'ops', 'op_read0', 'op_ref0')]
+
+    def _fetch(self, name, lo, count, size=None):
+        which, dtype, _ = self._ARRAYS[name]
+        out = np.zeros(count if size is None else size, dtype=dtype)
+        L = _lib.lib()
+        if count and L.bb_flat_fetch(self._handle, which, lo, count, _ptr(out)) != _lib.BB_OK:
+            raise RuntimeError('model builder: ' + L.bb_model_error().decode(errors='replace'))
+        return out
+
+    def __getattr__(self, name):
+        if name not in DeviceFlat._ARRAYS or self.__dict__.get('_handle') is None:
+            raise AttributeError(name)
+        total = int(getattr(self, self._ARRAYS[name][2])[-1])
+        arr = self._fetch(name, 0, total, max(total, 1))       # (one NUL / zero when empty, as FlatAlignments)
+        self.__dict__[name] = arr
+        return arr
+
+    def columns(self, a):
+        """FlatAlignments.columns, from alignment a's slices."""
+        r0, r1, f0, f1 = int(self.read_off[a]), int(self.read_off[a + 1]), int(self.ref_off[a]), int(self.ref_off[a + 1])
+        o0, o1 = int(self.ops_off[a]), int(self.ops_off[a + 1])
+        return _columns(self._fetch('read', r0, r1 - r0), self._fetch('ref', f0, f1 - f0), self._fetch('ops', o0, o1 - o0),
+                        self._fetch('op_read0', o0, o1 - o0), self._fetch('op_ref0', o0, o1 - o0))
+
+    def quals(self, a):
+        """FlatAlignments.quals, fetched for alignment a only."""
+        r0, r1 = int(self.read_off[a]), int(self.read_off[a + 1])
+        return self._fetch('qual', r0, r1 - r0)
+
+    def close(self):
+        if self._handle is not None:
+            _lib.lib().bb_flat_free(self._handle)
+            self._handle = None
+
+
+def _fastq_on_device(filename, output, dot_interval=1000):
+    """load_fastq's parse on the GPU (bb_fastq_parse) with its progress text and messages: the handle (bb_fastq_free)."""
+    from .engine import FastaFile
+    L = _lib.lib()
+    print('Loading reads', end='', file=output, flush=True)
+    get_compression_type(filename)      # (bzip2 and zip exit with its messages)
+    f = FastaFile(filename)
+    handle, n_rec, first = ctypes.c_void_p(), ctypes.c_int64(0), ctypes.c_int32(-1)
+    try:
+        rc = L.bb_fastq_parse(0, _ptr(f.data) if f.data.size else None, f.data.size, int(f.gzip), ctypes.byref(handle),
+                              ctypes.byref(n_rec), ctypes.byref(first))
+    finally:
+        f.close()
+    if rc != _lib.BB_OK:      # (the message names the record or the stage: "Error: ..."; the file goes in front of it)
+        msg = L.bb_model_error().decode(errors='replace')
+        sys.exit(f'\nError: {filename}: {msg[len("Error: "):]}' if msg.startswith('Error: ') else f'\nError: {filename}: {msg}')
+    if first.value != ord('@'):
+        L.bb_fastq_free(handle)
+        sys.exit('Error: {} is not FASTQ format'.format(filename))
+    print('.' * (n_rec.value // dot_interval), file=output, flush=True)
+    return handle
+
+
+def _touched_contigs(ref_ids, ref_names, refs):
+    """The contigs of reference ids ref_ids, concatenated once each: (offset of each id or -1 when refs lacks it, length
+    of each id, the bytes, their total)."""
+    contig_at = np.full(max(len(ref_names), 1), -1, dtype=np.int64)
+    contig_len = np.zeros(max(len(ref_names), 1), dtype=np.int64)
+    parts, pos = [], 0
+    for rid in np.unique(ref_ids).tolist():
+        seq = refs.get(ref_names[rid])
+        if seq is not None:
+            parts.append(seq.encode('latin-1'))
+            contig_at[rid], contig_len[rid] = pos, len(parts[-1])
+            pos += len(parts[-1])
+    return contig_at, contig_len, np.frombuffer(b''.join(parts) or b'\0', dtype=np.uint8), pos
+
+
+class _HostInputs(object):
+    """A builder's reads and chosen alignments on the host route."""
+
+    def __init__(self, reads, alignments, refs):
+        self.reads, self.alignments, self.refs, self.n = reads, alignments, refs, len(alignments)
+
+    def flatten(self, output, dot_interval):
+        return FlatAlignments(self.alignments, self.reads, self.refs, output, dot_interval)
+
+    def close(self):
+        pass
+
+
+class _DeviceInputs(object):
+    """A builder's reads (parsed on the GPU) and chosen PAF records on the device route, with load_fastq's and
+    load_alignments' progress text and messages; flatten() gathers the DeviceFlat.  close() releases everything."""
+
+    def __init__(self, args, refs, output, dot_interval=1000):
+        self.refs, self.fastq, self.records, self.flat = refs, None, None, None
+        try:
+            self.fastq = _fastq_on_device(args.reads, output)
+            print('Loading alignments', end='', file=output, flush=True)
+            self.records = _parse_records(args.alignment, 'paf', args.max_alignments)
+            self.view, n, self.ref_names, self.read_names, self.a = _record_arrays(self.records)
+            print('.' * (n // dot_interval), file=output, flush=True)
+            print('Choosing best alignment per read', end='', file=output, flush=True)
+            best = _best_per_read(self.a, n)
+            self.chosen = _usable(best, self.a['columns'][best], self.a['columns'][best].astype(np.int64) - self.a['nm'][best])
+            print('.' * (len(self.chosen) // dot_interval), file=output, flush=True)
+            self.n = len(self.chosen)
+        except BaseException:
+            self.close()
+            raise
+
+    def flatten(self, output, dot_interval):
+        L, a, chosen = _lib.lib(), self.a, self.chosen.astype(np.int64)
+        print('Processing alignments', end='', file=output, flush=True)
+        contig_at, contig_len, contigs, pos = _touched_contigs(a['ref_id'][chosen], self.ref_names, self.refs)
+        handle, failed = ctypes.c_void_p(), np.zeros(2, dtype=np.int64)
+        rc = L.bb_flat_build(self.fastq, ctypes.byref(self.view), len(chosen), _ptr(chosen), _ptr(contig_at), _ptr(contig_len),
+                             _ptr(contigs), pos, ctypes.byref(handle), _ptr(failed))
+        if rc != _lib.BB_OK:
+            i, kind = int(failed[0]), int(failed[1])
+            if kind == 0:
+                sys.exit('\n' + L.bb_model_error().decode(errors='replace'))
+            print('.' * (i // dot_interval), end='', file=output, flush=True)
+            read, ref = self.read_names[a['read_id'][chosen[i]]], self.ref_names[a['ref_id'][chosen[i]]]
+            if kind == 1:
+                sys.exit(f'\nError: could not find read {read}\nare you sure your read file and alignment file match?')
+            if kind == 2:
+                sys.exit(f'\nError: could not find reference {ref}\nare you sure your reference file and alignment file match?')
+            sys.exit(f'\nError: read {read} has bytes outside ASCII in its sequence or qualities')
+        self.flat = DeviceFlat(handle)
+        L.bb_fastq_free(self.fastq)
+        self.fastq = None
+        print('.' * (self.n // dot_interval), file=output, flush=True)
+        return self.flat
+
+    def close(self):
+        L = _lib.lib()
+        if self.flat is not None:
+            self.flat.close()
+            self.flat = None
+        if self.fastq is not None:
+            L.bb_fastq_free(self.fastq)
+            self.fastq = None
+        if self.records is not None:
+            L.bb_aln_free(self.records)
+            self.records = None
+
+
+def _inputs(args, refs, output, need_qual):
+    """A builder's inputs on the route device_route chooses."""
+    if device_route(args, alignment_format(args.alignment)):
+        return _DeviceInputs(args, refs, output)
+    reads, alignments = load_inputs(args, refs, output, need_qual)
+    return _HostInputs(reads, alignments, refs)
 
 
 def _ptr(a):
@@ -389,16 +613,20 @@ def _count(which, flat, k, max_del=0, device=0, cap=None, ovf_cap=None):
         ovf = [np.empty(ovf_cap, dtype=np.int32) for _ in range(3)]
         overall = np.zeros(N_Q, dtype=np.uint64)
         n_entries, n_ovf = ctypes.c_int64(0), ctypes.c_int64(0)
-        common = [_ptr(flat.ref), _ptr(flat.ref_off), _ptr(flat.ops), _ptr(flat.op_read0), _ptr(flat.op_ref0), _ptr(flat.ops_off),
-                  cap, _ptr(keys), _ptr(first), _ptr(counts), ctypes.byref(n_entries)]
+        if isinstance(flat, DeviceFlat):
+            read, qual, ref, ops, p0, r0 = flat.device_pointers
+        else:
+            read, qual, ref, ops, p0, r0 = (_ptr(x) for x in (flat.read, flat.qual, flat.ref, flat.ops, flat.op_read0, flat.op_ref0))
+        common = [ref, _ptr(flat.ref_off), ops, p0, r0, _ptr(flat.ops_off), cap, _ptr(keys), _ptr(first), _ptr(counts),
+                  ctypes.byref(n_entries)]
         tail = [ovf_cap, _ptr(ovf[0]), _ptr(ovf[1]), _ptr(ovf[2]), ctypes.byref(n_ovf)]
         if which == 'kmers':
-            rc = L.bb_count_kmer_alternatives(device, k, flat.n, _ptr(flat.read), _ptr(flat.read_off), *common, *tail)
+            rc = L.bb_count_kmer_alternatives(device, k, flat.n, read, _ptr(flat.read_off), *common, *tail)
         elif which == 'kmers_wide':
-            rc = L.bb_count_kmer_alternatives_wide(device, k, flat.n, _ptr(flat.read), _ptr(flat.read_off), *common, *tail)
+            rc = L.bb_count_kmer_alternatives_wide(device, k, flat.n, read, _ptr(flat.read_off), *common, *tail)
         else:
-            rc = L.bb_count_cigar_qscores(device, k, max_del, flat.n, _ptr(flat.read), _ptr(flat.qual), _ptr(flat.read_off),
-                                          *common, _ptr(overall), *tail)
+            rc = L.bb_count_cigar_qscores(device, k, max_del, flat.n, read, qual, _ptr(flat.read_off), *common, _ptr(overall),
+                                          *tail)
         if rc == _lib.BB_ERR_CAPACITY:
             if n_ovf.value > ovf_cap:
                 ovf_cap = int(n_ovf.value) + 16
@@ -490,13 +718,20 @@ def _error_model_lines_sparse(args, flat, k):
 def make_error_model(args, output=sys.stderr, dot_interval=1000):
     """error_model.py:31-83."""
     refs = load_fasta(args.reference)[0]
-    reads, alignments = load_inputs(args, refs, output, need_qual=False)
-    if len(alignments) == 0:
+    inputs = _inputs(args, refs, output, need_qual=False)
+    try:
+        _error_model(args, inputs, output, dot_interval)
+    finally:
+        inputs.close()
+
+
+def _error_model(args, inputs, output, dot_interval):
+    if inputs.n == 0:
         sys.exit('Error: no usable alignments')
     k = args.k_size
     if k > MAX_K_WIDE:
         sys.exit(f'Error: error models with k > {MAX_K_WIDE} are not supported by badread_b200')
-    flat = FlatAlignments(alignments, reads, refs, output, dot_interval)
+    flat = inputs.flatten(output, dot_interval)
     if k > MAX_K_DENSE:
         print(_error_model_lines_sparse(args, flat, k))
         return
@@ -562,11 +797,18 @@ def print_qscore_fractions(cigar, qscores, min_occur):
 def make_qscore_model(args, output=sys.stderr, dot_interval=1000):
     """qscore_model.py:78-161."""
     refs = load_fasta(args.reference)[0]
-    reads, alignments = load_inputs(args, refs, output, need_qual=True)
-    if len(alignments) == 0:
+    inputs = _inputs(args, refs, output, need_qual=True)
+    try:
+        _qscore_model(args, inputs, output, dot_interval)
+    finally:
+        inputs.close()
+
+
+def _qscore_model(args, inputs, output, dot_interval):
+    if inputs.n == 0:
         sys.exit('Error: no usable alignments')
     assert args.k_size % 2 == 1     # an odd size has a middle base to take the qscore from
-    flat = FlatAlignments(alignments, reads, refs, output, dot_interval)
+    flat = inputs.flatten(output, dot_interval)
     keys, first, counts, overall, ovf = _count('cigars', flat, args.k_size, args.max_del)
     table = {}          # cigar -> [histogram, first occurrence]
     for key, stamp, hist in zip(keys.tolist(), first.tolist(), counts):
@@ -576,8 +818,8 @@ def make_qscore_model(args, output=sys.stderr, dot_interval=1000):
     cache = {}
     for a, i, kk in zip(*(o.tolist() for o in ovf)):    # CIGARs longer than a key holds (or odd quality characters)
         if a not in cache:
-            cache[a] = flat.columns(a)
-        _, _, sym, dcount, _, _, lead = cache[a]
+            cache[a] = flat.columns(a), flat.quals(a)
+        (_, _, sym, dcount, _, _, lead), quals = cache[a]
         odd_quality = kk < 0
         kk = abs(kk)
         parts = ['D' * min(lead, args.max_del)] if i == 0 else []
@@ -586,7 +828,7 @@ def make_qscore_model(args, output=sys.stderr, dot_interval=1000):
             if j + 1 < kk:
                 parts.append('D' * min(int(dcount[i + j]), args.max_del))
         cigar = ''.join(parts)
-        q = int(flat.qual[flat.read_off[a] + i + (kk - 1) // 2]) - 33
+        q = int(quals[i + (kk - 1) // 2]) - 33
         if odd_quality:
             sys.exit(f'Error: quality character {chr(q + 33)!r} outside the Phred+33 range')
         stamp = (a << 36) | (((kk - 1) // 2) << 32) | i

@@ -451,7 +451,9 @@ BB_API int bb_bam_layout_sharded(int32_t n_shards, const bb_plan_view *const *vi
  * window size (negative for a bad quality character) in ovf_*; the caller evaluates those itself.  table_cap (a power of two)
  * slots are used on the device and bound the number of distinct keys; BB_ERR_CAPACITY if the table or the overflow list is
  * too small (*n_ovf then holds the required overflow capacity).  bb_model_error() describes the last failure of the calling
- * thread.  No bb_ctx is involved: the calls allocate and release what they need on `device`. */
+ * thread.  No bb_ctx is involved: the calls allocate and release what they need on `device`.  read, qual, ref, ops,
+ * op_read0 and op_ref0 may be host memory, copied to the device for the call, or device memory of `device` (a bb_flat_view's
+ * arrays), used in place; the three offset arrays are host memory. */
 BB_API int bb_count_kmer_alternatives(int device, int k, int32_t n_aln, const uint8_t *read, const int64_t *read_off,
                                const uint8_t *ref, const int64_t *ref_off, const uint32_t *ops, const int32_t *op_read0,
                                const int32_t *op_ref0, const int64_t *ops_off, int64_t table_cap, uint64_t *keys_out,
@@ -483,7 +485,14 @@ BB_API const char *bb_model_error(void);
  * without SEQ has none, has_qual[i] = 0 without QUAL, full[i] = SEQ present and no H clip.  Reads and references are
  * numbered in order of first appearance (references of a BAM header or of SAM @SQ lines first).
  * BB_ERR_ARG with bb_model_error() = the message to exit with: "Error: no CIGAR string found" (a mapped record with
- * CIGAR '*'), "Error: no alignment score" (no AS:i), an N or P op (names the read), or malformed input. */
+ * CIGAR '*'), "Error: no alignment score" (no AS:i), an N or P op (names the read), or malformed input.
+ * With is_bam = 2 (BB_ALN_PAF) data is PAF text, read as model_builders.load_alignments reads it: '\n', "\r\n" and a lone
+ * '\r' end lines, each line is stripped (str.strip()'s ASCII set) and split on '\t', and every line is a record (at most
+ * max_records lines are parsed).  read_start / read_end / ref_start / ref_end are columns 3, 4, 8 and 9 as written,
+ * columns = column 11, nm = column 11 - column 10, flag 0x10 on strand '-', score = the last AS:i: tag, and the CIGAR the
+ * last cg:Z: tag's runs (a digit run followed by a letter or '='; other bytes are skipped) with M I D as BAM's codes and
+ * every other letter as 15.  BB_ERR_ARG: "Error: alignment file does not seem to be in PAF format" (fewer than 11
+ * columns), "Error: no CIGAR string found", "Error: no alignment score", or a field that is not an integer. */
 typedef struct bb_aln_set bb_aln_set;
 typedef struct bb_aln_view {
     int64_t n_records;
@@ -499,6 +508,46 @@ typedef struct bb_aln_view {
 BB_API int bb_aln_parse(const uint8_t *data, int64_t n, int is_bam, int64_t max_records, bb_aln_set **set);
 BB_API int bb_aln_view_get(const bb_aln_set *set, bb_aln_view *view);   /* valid until bb_aln_free */
 BB_API int bb_aln_free(bb_aln_set *set);
+#define BB_ALN_PAF 2
+
+/* The model builders' device route for FASTQ reads (model_builders.DeviceFlat).  bb_device_count: the CUDA devices the
+ * library sees (0 when there are none or no driver).
+ * bb_fastq_parse: data[0..n) (host memory: the file as it is; is_gzip: a gzip stream, BGZF or not, inflated on the device
+ * as bb_gzip_decompress does) parsed on `device` as model_builders.load_fastq parses it (csrc/bb_fastq.cuh).  *first_byte:
+ * the first byte of the inflated text (-1 when it is empty); only a text that starts with '@' is parsed, into *n_records
+ * records whose name, sequence and quality spans stay on the device and whose names come to the host.  BB_ERR_ARG with
+ * bb_model_error() naming the record for a header without a name or a record the file ends in; BB_ERR_CAPACITY naming the
+ * stage and the bytes asked for when device memory runs out.  Device memory peaks at the inflater's peak, then at the text
+ * plus 56 bytes per record plus 8 per line.
+ * bb_flat_build: the flat arrays of bb_count_* on the device for n_aln alignments, records[i] of the bb_aln_view v (PAF):
+ * reads joined to FASTQ records by name (a repeated name: its last record), references at contig_at[ref id] of
+ * contigs[0..contigs_len) (-1: not loaded), contig_len[ref id] bytes long; the read, quality and reference slices with
+ * Python's slice semantics, the reference reverse-complemented on '-', each padded with NUL to the CIGAR's length
+ * (model_builders.FlatAlignments).  BB_ERR_ARG with failed[0] = the first alignment whose read (failed[1] = 1) or reference
+ * (2) is missing, checked in that order per alignment, or the first whose read holds a byte >= 0x80 in its sequence or
+ * qualities (3).  On success the FASTQ's text and record table are released (its names stay until bb_fastq_free).  Device
+ * memory then holds the text and record table plus the flat arrays: 2 bytes per read column, 1 per reference column and 12
+ * per CIGAR run, and the uploaded contigs.
+ * bb_flat_fetch copies elements [lo, lo + count) of array `which` (0 read, 1 qual, 2 ref, 3 ops, 4 op_read0, 5 op_ref0)
+ * to host memory. */
+typedef struct bb_fastq_set bb_fastq_set;
+typedef struct bb_flat_set bb_flat_set;
+typedef struct bb_flat_view {
+    int32_t n;                                                   /* alignments */
+    const uint8_t *read, *qual, *ref;                            /* device memory */
+    const uint32_t *ops; const int32_t *op_read0, *op_ref0;      /* device memory */
+    const int64_t *read_off, *ref_off, *ops_off;                 /* host memory, [n + 1] */
+} bb_flat_view;
+BB_API int bb_device_count(void);
+BB_API int bb_fastq_parse(int device, const uint8_t *data, int64_t n, int is_gzip, bb_fastq_set **set, int64_t *n_records,
+                          int32_t *first_byte);
+BB_API int bb_fastq_free(bb_fastq_set *set);
+BB_API int bb_flat_build(bb_fastq_set *fastq, const bb_aln_view *v, int32_t n_aln, const int64_t *records, const int64_t *contig_at,
+                         const int64_t *contig_len, const uint8_t *contigs, int64_t contigs_len, bb_flat_set **flat,
+                         int64_t *failed);
+BB_API int bb_flat_view_get(const bb_flat_set *flat, bb_flat_view *view);   /* valid until bb_flat_free */
+BB_API int bb_flat_fetch(const bb_flat_set *flat, int which, int64_t lo, int64_t count, void *dst);
+BB_API int bb_flat_free(bb_flat_set *flat);
 
 #ifdef __cplusplus
 }
