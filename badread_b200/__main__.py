@@ -2,7 +2,9 @@
 Command line of badread_b200: `python -m badread_b200 simulate ...` with the flags, defaults and validation
 messages of `badread simulate` (/root/reference/badread/__main__.py:83-147, 239-336). Additive flags: --gpus,
 --batch_reads. `error_model` and `qscore_model` take the reference's arguments, and their --alignment may also be SAM or
-BAM (then --reads is optional). The plotting subcommand of Badread is outside this package's scope.
+BAM (then --reads is optional). `plot` takes the reference's arguments, computes the window series on the GPU and
+does not draw: --no_plot prints what the reference prints, and the additive --windows FILE writes the series as a
+table (its --alignment may also be SAM or BAM).
 
 Derived from Badread (Copyright 2018 Ryan Wick, rrwick@gmail.com, https://github.com/rrwick/Badread), which is free
 software under the GNU General Public License version 3 or later; this file mirrors the named parts of the
@@ -29,6 +31,12 @@ def main(output=sys.stderr):
     elif args.subparser_name == 'qscore_model':
         from .model_builders import make_qscore_model
         make_qscore_model(args, output=output)
+    elif args.subparser_name == 'plot':
+        if not args.no_plot and args.windows is None:
+            sys.exit('Error: badread_b200 does not draw plots: write the window series with --windows FILE, or use '
+                     '--no_plot')
+        from .plot import plot_window_identity
+        plot_window_identity(args, output=sys.stdout)
     else:
         sys.exit(f'Error: the {args.subparser_name} command is not part of badread_b200 (use Badread itself)')
 
@@ -40,7 +48,7 @@ def parse_args(args):
     simulate_subparser(subparsers)
     model_subparser(subparsers, 'error_model', 'Build a Badread error model', 7)
     model_subparser(subparsers, 'qscore_model', 'Build a Badread qscore model', 9)
-    subparsers.add_parser('plot', add_help=False)
+    plot_subparser(subparsers)
     parser.add_argument('--version', action='version', version='Badread v' + __version__)
     if len(args) == 0:
         parser.print_help(file=sys.stderr)
@@ -80,6 +88,32 @@ def model_subparser(subparsers, name, description, default_k):
                               help='CIGARs which occur less than this many times will not be included in the model')
         optional.add_argument('--max_output', type=int, default=10000,
                               help='The outputted model will be limited to this many lines')
+    group.add_argument('--version', action='version', version='Badread v' + __version__)
+
+
+def positive_int(text):
+    value = int(text)
+    if value < 1:
+        raise argparse.ArgumentTypeError(f'must be at least 1: {text}')
+    return value
+
+
+def plot_subparser(subparsers):
+    """The arguments of `badread plot` (__main__.py:212-236 of the reference) and --windows; --window must be at least 1."""
+    group = subparsers.add_parser('plot', description='View read identities over a sliding window')
+    required = group.add_argument_group('Required arguments')
+    required.add_argument('--reference', type=str, required=True, help='Reference FASTA file')
+    required.add_argument('--reads', type=str, required=True, help='FASTQ of real reads')
+    required.add_argument('--alignment', type=str, required=True,
+                          help='Alignment of reads to the reference: PAF with cg:Z: and AS:i: tags, or SAM / BAM with '
+                               'AS:i: tags (told apart by content)')
+    optional = group.add_argument_group('Optional arguments')
+    optional.add_argument('--window', type=positive_int, default=100, help='Window size in bp')
+    optional.add_argument('--qual', action='store_true', help='Include qscores in plot (default: only show identity)')
+    optional.add_argument('--no_plot', action='store_true', help='Do not display plots (for testing purposes)')
+    optional.add_argument('--windows', type=str,
+                          help='Write the window series to this file as tab-separated lines: read name, position, '
+                               'identity and, with --qual, mean qscore (BGZF when the name ends in .gz)')
     group.add_argument('--version', action='version', version='Badread v' + __version__)
 
 

@@ -185,10 +185,14 @@ def lib():
         'bb_device_count': (c.c_int, []),
         'bb_fastq_parse': (c.c_int, [c.c_int, vp, i64, c.c_int, P(vp), P(i64), P(i32)]),
         'bb_fastq_free': (c.c_int, [vp]),
-        'bb_flat_build': (c.c_int, [vp, P(AlnView), i32, vp, vp, vp, vp, i64, P(vp), vp]),
+        'bb_flat_build': (c.c_int, [vp, P(AlnView), i32, vp, vp, vp, vp, i64, P(vp), vp, vp]),
         'bb_flat_view_get': (c.c_int, [vp, P(FlatView)]),
         'bb_flat_fetch': (c.c_int, [vp, c.c_int, i64, i64, vp]),
         'bb_flat_free': (c.c_int, [vp]),
+        'bb_window_series': (c.c_int, [c.c_int, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, i64, c.c_int, i32, i32, vp, vp,
+                                       P(i64)]),
+        'bb_window_line_bound': (i64, [i64]),
+        'bb_window_format': (c.c_int, [i32, vp, vp, vp, vp, vp, vp, i64, i64, vp, i64, P(i64)]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(L, name)
@@ -211,4 +215,5 @@ EXPORTED_SYMBOLS = ['bb_create', 'bb_destroy', 'bb_last_error', 'bb_version', 'b
                     'bb_fetch_last_batch_results', 'bb_bam_build', 'bb_bam_compress_device', 'bb_bam_fetch_records',
                     'bb_bam_compress', 'bb_bam_layout_sharded', 'bb_fasta_parse', 'bb_fasta_headers', 'bb_fasta_reference',
                     'bb_download_reference', 'bb_gzip_decompress', 'bb_last_gzip_stats', 'bb_device_count', 'bb_fastq_parse',
-                    'bb_fastq_free', 'bb_flat_build', 'bb_flat_view_get', 'bb_flat_fetch', 'bb_flat_free']
+                    'bb_fastq_free', 'bb_flat_build', 'bb_flat_view_get', 'bb_flat_fetch', 'bb_flat_free', 'bb_window_series',
+                    'bb_window_line_bound', 'bb_window_format']

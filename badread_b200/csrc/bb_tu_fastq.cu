@@ -225,7 +225,7 @@ extern "C" int bb_fastq_free(bb_fastq_set *F) {
 
 extern "C" int bb_flat_build(bb_fastq_set *F, const bb_aln_view *v, int32_t n_aln, const int64_t *records, const int64_t *contig_at,
                              const int64_t *contig_len, const uint8_t *contigs, int64_t contigs_len, bb_flat_set **out,
-                             int64_t *failed) {
+                             int64_t *failed, int64_t *slice_len) {
     bbm_set_error("");
     if (!F || !v || n_aln < 0 || (n_aln && (!records || !contig_at || !contig_len)) || contigs_len < 0 ||
         (contigs_len && !contigs) || !out || !failed || (n_aln && !F->text)) {
@@ -267,6 +267,18 @@ extern "C" int bb_flat_build(bb_fastq_set *F, const bb_aln_view *v, int32_t n_al
             check(cudaMemcpy(flat->ops, ops.data(), (size_t)n_ops * 4, cudaMemcpyHostToDevice), "cudaMemcpy");
             check(cudaMemcpy(flat->op_read0, p0.data(), (size_t)n_ops * 4, cudaMemcpyHostToDevice), "cudaMemcpy");
             check(cudaMemcpy(flat->op_ref0, r0.data(), (size_t)n_ops * 4, cudaMemcpyHostToDevice), "cudaMemcpy");
+        }
+        if (slice_len && n_aln) {   // (the records' spans: the slices' lengths before fq_k_gather pads or truncates them)
+            std::vector<FastqRec> recs((size_t)F->n_rec);
+            d2h(recs.data(), F->recs, F->n_rec);
+            for (int32_t i = 0; i < n_aln; i++) {
+                const FastqAln &A = alns[(size_t)i];
+                const FastqRec &R = recs[(size_t)A.rec];
+                int64_t lo;
+                slice_len[3 * (int64_t)i] = fq_slice(R.seq_hi - R.seq_lo, A.read_start, A.read_end, &lo);
+                slice_len[3 * (int64_t)i + 1] = fq_slice(R.qual_hi - R.qual_lo, A.read_start, A.read_end, &lo);
+                slice_len[3 * (int64_t)i + 2] = fq_slice(A.contig_len, A.ref_start, A.ref_end, &lo);
+            }
         }
         const FastqAln *d_alns = upload(S, alns.data(), n_aln, "the alignment descriptors");
         const int64_t *d_read_off = upload(S, flat->read_off.data(), n_aln + 1, "the alignment descriptors");

@@ -150,12 +150,17 @@ def alignment_format(filename):
 
 
 class SamAlignment(object):
-    """The chosen alignment of a read from a SAM / BAM record: the attributes of Alignment that FlatAlignments reads."""
-    __slots__ = ('read_name', 'read_start', 'read_end', 'strand', 'ref_name', 'ref_start', 'ref_end', 'runs')
+    """The chosen alignment of a read from a SAM / BAM record: the attributes of Alignment that FlatAlignments reads, and
+    its identity for Alignment's repr."""
+    __slots__ = ('read_name', 'read_start', 'read_end', 'strand', 'ref_name', 'ref_start', 'ref_end', 'runs',
+                 'percent_identity')
 
-    def __init__(self, read_name, read_start, read_end, strand, ref_name, ref_start, ref_end, runs):
+    def __init__(self, read_name, read_start, read_end, strand, ref_name, ref_start, ref_end, runs, percent_identity):
         self.read_name, self.read_start, self.read_end, self.strand = read_name, read_start, read_end, strand
         self.ref_name, self.ref_start, self.ref_end, self.runs = ref_name, ref_start, ref_end, runs
+        self.percent_identity = percent_identity
+
+    __repr__ = Alignment.__repr__
 
 
 def _view_array(ptr, n, dtype):
@@ -274,6 +279,8 @@ def load_sam_alignments(filename, fmt, max_alignments, reads, refs, need_qual, o
         i = int(best[k])
         matches[k] = _count_matches(i, a, cigar, cigar_off, whole_read(i), refs.get(ref_names[a['ref_id'][i]]))
     keep = _usable(best, a['columns'][best], matches)
+    with np.errstate(divide='ignore', invalid='ignore'):
+        identity_of = dict(zip(best.tolist(), (100.0 * matches / a['columns'][best].astype(np.int64)).tolist()))
     chosen = []
     for i in keep.tolist():
         name = read_names[a['read_id'][i]]
@@ -284,7 +291,7 @@ def load_sam_alignments(filename, fmt, max_alignments, reads, refs, need_qual, o
         if strand == '-':
             runs.reverse()
         chosen.append(SamAlignment(name, int(a['read_start'][i]), int(a['read_end'][i]), strand, ref_names[a['ref_id'][i]],
-                                   int(a['ref_start'][i]), int(a['ref_end'][i]), runs))
+                                   int(a['ref_start'][i]), int(a['ref_end'][i]), runs, identity_of[i]))
         if len(chosen) % dot_interval == 0:
             print('.', end='', file=output, flush=True)
     print('', file=output, flush=True)
@@ -545,13 +552,16 @@ class _DeviceInputs(object):
             self.close()
             raise
 
-    def flatten(self, output, dot_interval):
+    def flatten(self, output, dot_interval, slice_len=None):
+        """The DeviceFlat of the chosen alignments; slice_len (an int64 array (n, 3), or None) gets the lengths of
+        each alignment's sequence, quality and reference slices before they are fitted to its CIGAR."""
         L, a, chosen = _lib.lib(), self.a, self.chosen.astype(np.int64)
         print('Processing alignments', end='', file=output, flush=True)
         contig_at, contig_len, contigs, pos = _touched_contigs(a['ref_id'][chosen], self.ref_names, self.refs)
         handle, failed = ctypes.c_void_p(), np.zeros(2, dtype=np.int64)
         rc = L.bb_flat_build(self.fastq, ctypes.byref(self.view), len(chosen), _ptr(chosen), _ptr(contig_at), _ptr(contig_len),
-                             _ptr(contigs), pos, ctypes.byref(handle), _ptr(failed))
+                             _ptr(contigs), pos, ctypes.byref(handle), _ptr(failed),
+                             None if slice_len is None else _ptr(slice_len))
         if rc != _lib.BB_OK:
             i, kind = int(failed[0]), int(failed[1])
             if kind == 0:

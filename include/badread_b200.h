@@ -525,7 +525,9 @@ BB_API int bb_aln_free(bb_aln_set *set);
  * Python's slice semantics, the reference reverse-complemented on '-', each padded with NUL to the CIGAR's length
  * (model_builders.FlatAlignments).  BB_ERR_ARG with failed[0] = the first alignment whose read (failed[1] = 1) or reference
  * (2) is missing, checked in that order per alignment, or the first whose read holds a byte >= 0x80 in its sequence or
- * qualities (3).  On success the FASTQ's text and record table are released (its names stay until bb_fastq_free).  Device
+ * qualities (3).  slice_len (may be NULL) gets, per alignment, 3 lengths before any padding or truncation: of the read's
+ * sequence slice, of its quality slice and of the reference slice (`badread_b200 plot` refuses alignments whose CIGAR
+ * does not fit them).  On success the FASTQ's text and record table are released (its names stay until bb_fastq_free).  Device
  * memory then holds the text and record table plus the flat arrays: 2 bytes per read column, 1 per reference column and 12
  * per CIGAR run, and the uploaded contigs.
  * bb_flat_fetch copies elements [lo, lo + count) of array `which` (0 read, 1 qual, 2 ref, 3 ops, 4 op_read0, 5 op_ref0)
@@ -544,10 +546,36 @@ BB_API int bb_fastq_parse(int device, const uint8_t *data, int64_t n, int is_gzi
 BB_API int bb_fastq_free(bb_fastq_set *set);
 BB_API int bb_flat_build(bb_fastq_set *fastq, const bb_aln_view *v, int32_t n_aln, const int64_t *records, const int64_t *contig_at,
                          const int64_t *contig_len, const uint8_t *contigs, int64_t contigs_len, bb_flat_set **flat,
-                         int64_t *failed);
+                         int64_t *failed, int64_t *slice_len);
 BB_API int bb_flat_view_get(const bb_flat_set *flat, bb_flat_view *view);   /* valid until bb_flat_free */
 BB_API int bb_flat_fetch(const bb_flat_set *flat, int which, int64_t lo, int64_t count, void *dst);
 BB_API int bb_flat_free(bb_flat_set *flat);
+
+/* ---- `badread plot`'s window series (plot_window_identity.get_window_means of the reference; csrc/bb_plot.cuh).
+ * bb_window_series: for the alignments first_aln .. first_aln + n_pass - 1 of the flat arrays of bb_count_* (read, qual,
+ * ref, ops, op_read0 and op_ref0 host memory, copied for the call, or device memory of `device`, used in place; the
+ * offsets [n_aln + 1] host memory), each of read slice length L, the windows i = 0 .. L - window - 1 in order, the
+ * alignments one after the other: out_identity[] = 100 * (1 - S / window) with S the errors of read positions
+ * [i, i + window) (1 per mismatching M base and per I base, n at the read offset where a D run of n starts), and with
+ * want_qual out_qual[] = the sum of (quality byte - 33) over the window / window, both rounded as Python's float
+ * operations are.  *n_points = the windows written, sum of max(0, L - window); out_* host memory of that many doubles.
+ * The caller has checked every alignment: its M and I runs cover [0, L) exactly, no D run starts at L, its M runs lie
+ * inside its reference slice.  Device memory: 8 bytes per read position (16 with want_qual) plus 8 (16) per window, plus
+ * the inputs given in host memory.  BB_ERR_ARG for window < 1 or a range outside [0, n_aln); BB_ERR_CAPACITY naming
+ * what did not fit in device memory.
+ * bb_window_format: the table lines ("name\tposition\t%.4f identity[\t%.4f qscore]\n") of windows [lo, hi) of a
+ * series of n_aln alignments: alignment a's name names[name_off[a] .. name_off[a + 1]), its windows [point_off[a],
+ * point_off[a + 1]) of identity[] (and qual[], or NULL), at positions pos0[a], pos0[a] + 1, ...  Several host threads
+ * format into out; *out_len = the bytes written.  BB_ERR_CAPACITY when cap is less than (hi - lo) times
+ * bb_window_line_bound(the longest name), the most one line can take. */
+BB_API int bb_window_series(int device, int32_t n_aln, const uint8_t *read, const uint8_t *qual, const uint8_t *ref,
+                            const int64_t *read_off, const int64_t *ref_off, const uint32_t *ops, const int32_t *op_read0,
+                            const int32_t *op_ref0, const int64_t *ops_off, int64_t window, int want_qual, int32_t first_aln,
+                            int32_t n_pass, double *out_identity, double *out_qual, int64_t *n_points);
+BB_API int64_t bb_window_line_bound(int64_t name_len);
+BB_API int bb_window_format(int32_t n_aln, const char *names, const int64_t *name_off, const int64_t *pos0,
+                            const int64_t *point_off, const double *identity, const double *qual, int64_t lo, int64_t hi,
+                            char *out, int64_t cap, int64_t *out_len);
 
 #ifdef __cplusplus
 }
