@@ -94,6 +94,22 @@ class FlatView(ctypes.Structure):
                                                                            'read_off', 'ref_off', 'ops_off')]
 
 
+class EmLoadInfo(ctypes.Structure):
+    """bb_em_load_info (include/badread_b200.h)."""
+    _fields_ = [('k', ctypes.c_int32), ('index', ctypes.c_int32)] + \
+        [(f, ctypes.c_int64) for f in ('n_rows', 'n_entries', 'n_alts', 'pool_bytes', 'text_bytes')] + \
+        [('fallback', ctypes.c_uint32), ('reserved', ctypes.c_int32)] + \
+        [(f, ctypes.c_double) for f in ('ms_inflate', 'ms_parse', 'ms_align', 'ms_tables', 'ms_index', 'ms_total')]
+
+    def as_dict(self):
+        return {f: getattr(self, f) for f, _ in self._fields_ if f != 'reserved'}
+
+
+# bb_em_fallback: why bb_load_error_model_file left a file to the host loader
+EM_FALLBACK = {'number': 1, 'duplicate': 2, 'k': 4, 'base': 8, 'syntax': 16, 'cr': 32, 'long_alt': 64, 'alt_ends': 128,
+               'empty_line': 256, 'input': 512, 'size': 1024}
+
+
 BB_ALN_PAF = 2
 
 
@@ -129,6 +145,8 @@ def lib():
         'bb_download_reference': (c.c_int, [vp, i64, i64, vp]),
         'bb_upload_error_model': (c.c_int, [vp, c.c_int, c.c_int, vp, i64, i32, vp, vp, vp, vp, vp, i64]),
         'bb_upload_error_model_kmers': (c.c_int, [vp, c.c_int, i32, vp, vp, vp, vp, vp, vp, i64]),
+        'bb_load_error_model_file': (c.c_int, [vp, vp, i64, P(EmLoadInfo)]),
+        'bb_download_error_model': (c.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, vp]),
         'bb_upload_qscore_model': (c.c_int, [vp, c.c_int, i32, vp, vp, vp, vp]),
         'bb_upload_qscore_model_cigars': (c.c_int, [vp, c.c_int, i32, vp, vp, vp, vp, vp]),
         'bb_sequence_batch': (c.c_int, [vp, i32, vp, vp, vp, vp, i64, vp, vp, vp, vp, i64, P(i64)]),
@@ -216,4 +234,4 @@ EXPORTED_SYMBOLS = ['bb_create', 'bb_destroy', 'bb_last_error', 'bb_version', 'b
                     'bb_bam_compress', 'bb_bam_layout_sharded', 'bb_fasta_parse', 'bb_fasta_headers', 'bb_fasta_reference',
                     'bb_download_reference', 'bb_gzip_decompress', 'bb_last_gzip_stats', 'bb_device_count', 'bb_fastq_parse',
                     'bb_fastq_free', 'bb_flat_build', 'bb_flat_view_get', 'bb_flat_fetch', 'bb_flat_free', 'bb_window_series',
-                    'bb_window_line_bound', 'bb_window_format']
+                    'bb_window_line_bound', 'bb_window_format', 'bb_load_error_model_file', 'bb_download_error_model']

@@ -5,6 +5,7 @@
 #include <unistd.h>
 
 #include <algorithm>
+#include <chrono>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -220,6 +221,8 @@ struct bb_ctx {
     bool have_em = false, have_qm = false;
     BBErrorModelDev em{}; DevBuf em_k2r, em_rowoff, em_cum, em_flags, em_slots, em_pool, em_rowinfo;
     BBEmHashDev em_hash{}; DevBuf em_hentries;  // k-mer index as a hash table (bb_upload_error_model_kmers)
+    // the model installed by bb_load_error_model_file (em_loaded): what bb_download_error_model copies besides the tables
+    bool em_loaded = false; DevBuf em_probs, em_codes; bb_em_load_info em_info{};
     BBQScoreModelDev qm{}; DevBuf qm_hkeys, qm_hvals, qm_lkeys, qm_lpool, qm_rowoff, qm_scores, qm_cum;
 
     // Sub-batches: a batch is dealt out over the workers and their kernel chains run side by side on their own
@@ -611,6 +614,7 @@ extern "C" int bb_upload_error_model(bb_ctx *ctx, int k, int type, const int32_t
     if (k < 1 || k > 12 || (type != 0 && type != 1)) return set_err(ctx, BB_ERR_ARG, "error model: k must be 1..12");
     BB_CUDA(ctx, cudaSetDevice(ctx->device));
     ctx->em = BBErrorModelDev{};
+    ctx->em_loaded = false;
     ctx->em_hash = BBEmHashDev{};
     ctx->em.k = k; ctx->em.type = type;
     if (type == 1) {
@@ -638,6 +642,7 @@ extern "C" int bb_upload_error_model_kmers(bb_ctx *ctx, int k, int32_t n_rows, c
     if (!bb_build_em_hash(k, n_rows, kmer_codes, t, err)) return set_err(ctx, BB_ERR_ARG, err);
     BB_CUDA(ctx, cudaSetDevice(ctx->device));
     ctx->em = BBErrorModelDev{};
+    ctx->em_loaded = false;
     ctx->em_hash = BBEmHashDev{};
     ctx->have_em = false;
     int rc;
@@ -647,6 +652,123 @@ extern "C" int bb_upload_error_model_kmers(bb_ctx *ctx, int k, int32_t n_rows, c
     ctx->em_hash.entries = ctx->em_hentries.as<unsigned long long>(); ctx->em_hash.bits = t.bits;
     ctx->have_em = true;
     for (const auto &w : ctx->workers) w->uploaded = false;  // the fragment layout of a batch depends on k
+    return BB_OK;
+}
+
+// Takes ownership of a device allocation
+static void adopt(DevBuf &buf, void *p, size_t bytes) {
+    buf.release();
+    buf.p = p;
+    buf.cap = bytes;
+}
+
+extern "C" int bb_load_error_model_file(bb_ctx *ctx, const uint8_t *bytes, int64_t n, bb_em_load_info *info) {
+    if (!ctx || n < 0 || (n && !bytes) || !info) return set_err(ctx, BB_ERR_ARG, "bb_load_error_model_file: bad arguments");
+    BB_CUDA(ctx, cudaSetDevice(ctx->device));
+    for (const auto &w : ctx->workers) BB_CUDA(ctx, cudaStreamSynchronize(w->stream));
+    *info = bb_em_load_info{};
+    const auto t0 = std::chrono::steady_clock::now();
+    const cudaStream_t st = ctx->w0().stream;
+    // misc.get_compression_type's magic numbers: gzip (BGZF or not) is inflated here, bzip2 and zip are the host's to refuse
+    const bool gz = n >= 3 && bytes[0] == 0x1f && bytes[1] == 0x8b && bytes[2] == 0x08;
+    if ((n >= 3 && bytes[0] == 'B' && bytes[1] == 'Z' && bytes[2] == 'h') ||
+        (n >= 4 && bytes[0] == 'P' && bytes[1] == 'K' && bytes[2] == 3 && bytes[3] == 4)) {
+        info->fallback = BB_EM_FALLBACK_INPUT;
+        return BB_OK;
+    }
+    DevBuf text;
+    int64_t len = n;
+    if (gz) {
+        uint8_t *p = nullptr;
+        char msg[256];
+        bb_gzip_stats stats{};
+        const int rc = bbl_gzip_inflate_device(st, bytes, n, 0, &p, &len, &stats, msg, sizeof(msg));
+        if (rc == BB_ERR_ARG) {   // not a stream gzip.open reads either: the host loader reports it
+            info->fallback = BB_EM_FALLBACK_INPUT;
+            return BB_OK;
+        }
+        if (rc) return set_err(ctx, rc, msg);
+        text.p = p;
+        text.cap = (size_t)std::max<int64_t>(len, 16);
+    } else {
+        BB_CUDA(ctx, alloc_exact(text, (size_t)n));
+        if (n) BB_CUDA(ctx, cudaMemcpyAsync(text.p, bytes, (size_t)n, cudaMemcpyHostToDevice, st));
+        BB_CUDA(ctx, cudaStreamSynchronize(st));
+    }
+    auto t = std::chrono::steady_clock::now();
+    info->ms_inflate = std::chrono::duration<double, std::milli>(t - t0).count();
+    info->text_bytes = len;
+    BBEmLoadOut out;
+    char msg[256];
+    int rc = bbl_em_load(st, text.as<uint8_t>(), len, true, info, &out, msg, sizeof(msg));
+    text.release();
+    // the hash index for k > 12: BBEmHashTable's builder over the row codes made on the device
+    BBEmHashTable hash;
+    if (rc == BB_OK && !info->fallback && !out.kmer_to_row) {
+        std::vector<int64_t> codes((size_t)info->n_rows);
+        BB_CUDA(ctx, cudaMemcpy(codes.data(), out.codes, codes.size() * sizeof(int64_t), cudaMemcpyDeviceToHost));
+        std::string err;
+        if (!bb_build_em_hash(info->k, (int32_t)info->n_rows, codes.data(), hash, err)) info->fallback |= BB_EM_FALLBACK_DUPLICATE;
+    }
+    if (rc != BB_OK || info->fallback) {
+        bbl_em_load_free(&out);
+        return rc == BB_OK ? BB_OK : set_err(ctx, rc, msg);
+    }
+    ctx->have_em = false;
+    ctx->em = BBErrorModelDev{};
+    ctx->em_hash = BBEmHashDev{};
+    const size_t ne = (size_t)info->n_entries, nr = (size_t)info->n_rows;
+    if (out.kmer_to_row) {
+        adopt(ctx->em_k2r, out.kmer_to_row, ((size_t)1 << (2 * info->k)) * sizeof(int32_t));
+        info->index = 1;
+    } else {
+        if (const int urc = upload(ctx, st, ctx->em_hentries, hash.entries.data(), hash.entries.size())) {
+            bbl_em_load_free(&out);
+            return urc;
+        }
+        info->index = 2;
+    }
+    adopt(ctx->em_codes, out.codes, nr * sizeof(int64_t));
+    adopt(ctx->em_rowoff, out.row_off, (nr + 1) * sizeof(int32_t));
+    adopt(ctx->em_cum, out.cum, ne * sizeof(double));
+    adopt(ctx->em_probs, out.probs, ne * sizeof(double));
+    adopt(ctx->em_flags, out.flags, std::max<size_t>(ne, 1));
+    adopt(ctx->em_slots, out.slots, std::max<size_t>(ne * info->k, 1) * sizeof(uint32_t));
+    adopt(ctx->em_pool, out.pool, (size_t)std::max<int64_t>(info->pool_bytes, 1));
+    adopt(ctx->em_rowinfo, out.rowinfo, nr * sizeof(BBRowInfo));
+    BB_CUDA(ctx, cudaStreamSynchronize(st));
+    const auto t1 = std::chrono::steady_clock::now();
+    info->ms_index = std::chrono::duration<double, std::milli>(t1 - t).count() - info->ms_parse - info->ms_align - info->ms_tables;
+    info->ms_total = std::chrono::duration<double, std::milli>(t1 - t0).count();
+    ctx->em.k = info->k; ctx->em.type = 1;
+    ctx->em.kmer_to_row = info->index == 1 ? ctx->em_k2r.as<int32_t>() : nullptr;
+    ctx->em.row_off = ctx->em_rowoff.as<int32_t>();
+    ctx->em.cum = ctx->em_cum.as<double>(); ctx->em.flags = ctx->em_flags.as<uint8_t>();
+    ctx->em.slots = ctx->em_slots.as<uint32_t>(); ctx->em.pool = ctx->em_pool.as<uint8_t>();
+    ctx->em.rowinfo = ctx->em_rowinfo.as<BBRowInfo>();
+    if (info->index == 2) { ctx->em_hash.entries = ctx->em_hentries.as<unsigned long long>(); ctx->em_hash.bits = hash.bits; }
+    ctx->em_info = *info;
+    ctx->em_loaded = true;
+    ctx->have_em = true;
+    for (const auto &w : ctx->workers) w->uploaded = false;  // the fragment layout of a batch depends on k
+    return BB_OK;
+}
+
+extern "C" int bb_download_error_model(bb_ctx *ctx, int32_t *kmer_to_row, int64_t *kmer_codes, int32_t *row_off, double *cum,
+                                       double *probs, uint8_t *flags, uint32_t *slots, uint8_t *pool) {
+    if (!ctx) return BB_ERR_ARG;
+    if (!ctx->em_loaded) return set_err(ctx, BB_ERR_STATE, "bb_download_error_model: no model installed by bb_load_error_model_file");
+    const bb_em_load_info &I = ctx->em_info;
+    if (kmer_to_row && I.index != 1) return set_err(ctx, BB_ERR_ARG, "bb_download_error_model: the model has no dense index");
+    BB_CUDA(ctx, cudaSetDevice(ctx->device));
+    const size_t ne = (size_t)I.n_entries, nr = (size_t)I.n_rows;
+    const struct { void *dst; const DevBuf &src; size_t bytes; } parts[] = {
+        {kmer_to_row, ctx->em_k2r, ((size_t)1 << (2 * I.k)) * sizeof(int32_t)}, {kmer_codes, ctx->em_codes, nr * sizeof(int64_t)},
+        {row_off, ctx->em_rowoff, (nr + 1) * sizeof(int32_t)}, {cum, ctx->em_cum, ne * sizeof(double)},
+        {probs, ctx->em_probs, ne * sizeof(double)}, {flags, ctx->em_flags, ne}, {slots, ctx->em_slots, ne * I.k * sizeof(uint32_t)},
+        {pool, ctx->em_pool, (size_t)std::max<int64_t>(I.pool_bytes, 1)}};
+    for (const auto &p : parts)
+        if (p.dst && p.bytes) BB_CUDA(ctx, cudaMemcpy(p.dst, p.src.p, p.bytes, cudaMemcpyDeviceToHost));
     return BB_OK;
 }
 

@@ -75,5 +75,20 @@ int bbl_bgzf_inflate_device(cudaStream_t st, const uint8_t *in, int64_t n, uint8
 // Any gzip stream in host memory in[0..n) inflated the same way (bb_tu_gunzip.cu): through bbl_bgzf_inflate_device when
 // every member is BGZF, else in chunks of chunk_bytes (0: the default); *stats as bb_gzip_decompress reports them.
 struct bb_gzip_stats;
+// An error model file's text[0..n) in device memory to its tables (bb_em_load.cuh), in new device allocations that
+// bbl_em_load_free releases.  kmer_to_row[4^k] only when `dense` and k <= 12.  info->fallback set: nothing to install.
+struct BBEmLoadOut {
+    int32_t *kmer_to_row = nullptr;
+    int64_t *codes = nullptr;
+    int32_t *row_off = nullptr;
+    double *cum = nullptr, *probs = nullptr;
+    uint8_t *flags = nullptr;
+    uint32_t *slots = nullptr;
+    uint8_t *pool = nullptr;
+    BBRowInfo *rowinfo = nullptr;
+};
+int bbl_em_load(cudaStream_t st, const uint8_t *text, int64_t n, bool dense, bb_em_load_info *info, BBEmLoadOut *out,
+                char *msg, size_t msg_len);
+void bbl_em_load_free(BBEmLoadOut *out);
 int bbl_gzip_inflate_device(cudaStream_t st, const uint8_t *in, int64_t n, int64_t chunk_bytes, uint8_t **out,
                             int64_t *total, bb_gzip_stats *stats, char *msg, size_t msg_len);

@@ -22,7 +22,9 @@ assert _RESULT_DTYPE.itemsize == ctypes.sizeof(ReadResult)
 
 
 class EngineError(RuntimeError):
-    pass
+    def __init__(self, msg, code=None):
+        super().__init__(msg)
+        self.code = code   # the bb_status of the failed call
 
 
 def _ptr(a):
@@ -101,9 +103,10 @@ class FragmentBatch(object):
 
 
 class FastaFile(object):
-    """The bytes of a FASTA file as Engine.load_fasta takes them, read once for all the engines: the file as it is, in
-    page-locked memory (bb_host_alloc) so that it goes to the GPUs at the link's rate.  A gzip file, BGZF or not, is
-    inflated on the GPUs.  close() releases the memory."""
+    """The bytes of a FASTA file as Engine.load_fasta takes them (or of an error model file, for
+    Engine.load_error_model_file), read once for all the engines: the file as it is, in page-locked memory (bb_host_alloc)
+    so that it goes to the GPUs at the link's rate.  A gzip file, BGZF or not, is inflated on the GPUs.  close() releases
+    the memory."""
 
     def __init__(self, filename):
         self._lib = _lib.lib()
@@ -177,6 +180,7 @@ class Engine(object):
         self._seq_buf = self._qual_buf = None
         self._pinned = []
         self._bgzf_buf = None
+        self._em_installed = None   # the model object whose tables this GPU holds
 
     def close(self):
         if getattr(self, '_ctx', None):
@@ -193,7 +197,7 @@ class Engine(object):
     def _check(self, rc, what):
         if rc != 0:
             msg = self._lib.bb_last_error(self._ctx)
-            raise EngineError(f'{what} failed ({rc}): {msg.decode() if msg else ""}')
+            raise EngineError(f'{what} failed ({rc}): {msg.decode() if msg else ""}', rc)
 
     # ---- uploads
     def upload_reference(self, bases):
@@ -252,6 +256,10 @@ class Engine(object):
         measurement)."""
         if index not in ('auto', 'hash'):
             raise ValueError(f"index must be 'auto' or 'hash', not {index!r}")
+        if index == 'auto' and error_model is self._em_installed:   # (a DeviceErrorModel this GPU built)
+            self.error_model = error_model
+            return
+        self._em_installed = None
         t = error_model.to_device_tables()
         if t['type'] == 0:
             rc = self._lib.bb_upload_error_model(self._ctx, 1, 0, None, 0, 0, None, None, None, None, None, 0)
@@ -269,6 +277,45 @@ class Engine(object):
             name = 'bb_upload_error_model_kmers'
         self._check(rc, name)
         self.error_model = error_model
+        self._em_installed = error_model if index == 'auto' else None
+
+    def load_error_model_file(self, model_file, owner=None):
+        """Builds the tables ErrorModel(file) would build on this GPU, from the file's bytes, and installs them
+        (bb_load_error_model_file).  model_file: a FastaFile (one page-locked copy for all the engines) or a file name.
+        owner: the model object that stands for these tables (a DeviceErrorModel): set_error_model(owner) then uploads
+        nothing.  Returns the load's info (_lib.EmLoadInfo) as a dict; a non-zero info['fallback'] (_lib.EM_FALLBACK bits)
+        means the file is off the device loader's fast path and nothing was installed."""
+        own = not isinstance(model_file, FastaFile)
+        if own:
+            model_file = FastaFile(model_file)
+        try:
+            info = _lib.EmLoadInfo()
+            data = model_file.data
+            self._check(self._lib.bb_load_error_model_file(self._ctx, _ptr(data) if data.size else None, data.size,
+                                                           ctypes.byref(info)), 'bb_load_error_model_file')
+        finally:
+            if own:
+                model_file.close()
+        out = info.as_dict()
+        if not out['fallback']:
+            self.error_model = owner
+            self._em_installed = owner
+        return out
+
+    def download_error_model(self, info):
+        """The tables the last load_error_model_file installed (bb_download_error_model), as ErrorModel._tables holds
+        them; info is what that call returned."""
+        k, nr, ne = info['k'], info['n_rows'], info['n_entries']
+        t = {'row_off': np.zeros(nr + 1, np.int32), 'cum': np.zeros(ne, np.float64), 'flags': np.zeros(ne, np.uint8),
+             'slots': np.zeros(ne * k, np.uint32), 'pool': np.zeros(max(info['pool_bytes'], 1), np.uint8),
+             'probs': np.zeros(ne, np.float64), 'kmer_codes': np.zeros(nr, np.int64)}
+        if info['index'] == 1:
+            t['kmer_to_row'] = np.zeros(4 ** k, np.int32)
+        self._check(self._lib.bb_download_error_model(self._ctx, _ptr(t.get('kmer_to_row')), _ptr(t['kmer_codes']),
+                                                      _ptr(t['row_off']), _ptr(t['cum']), _ptr(t['probs']),
+                                                      _ptr(t['flags']), _ptr(t['slots']), _ptr(t['pool'])),
+                    'bb_download_error_model')
+        return t
 
     def set_qscore_model(self, qscore_model):
         t = qscore_model.to_device_tables()

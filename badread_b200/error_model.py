@@ -257,6 +257,72 @@ class ErrorModel(object):
         return alt
 
 
+class DeviceErrorModel(ErrorModel):
+    """An error model file loaded by the engines themselves: each one builds the tables from one page-locked copy of the
+    file's bytes on its GPU and keeps them there (Engine.load_error_model_file), so the file is never parsed on the host.
+    It prints what the host loader prints.  `_tables` (and with it `alternatives`, `probabilities`, `to_device_tables` and
+    `save_tables`) is copied from the first engine on first use, which must then still hold these tables (be open, with no other model
+    set since).  `info` is that engine's
+    load info (_lib.EmLoadInfo as a dict)."""
+
+    @classmethod
+    def load(cls, filename, engines, output=sys.stderr):
+        """The model built on every engine, or None when the file is off the device loader's fast path (or cannot be
+        read): then nothing was printed and ErrorModel(filename) loads it, with its messages."""
+        from .engine import EngineError, FastaFile, run_each
+        try:
+            data = FastaFile(filename)
+        except OSError:
+            return None
+        model = cls.__new__(cls)
+        infos = [None] * len(engines)
+
+        def load(g):
+            infos[g] = engines[g].load_error_model_file(data, owner=model)
+
+        try:
+            run_each(len(engines), load)
+        except EngineError as e:
+            if e.code != _lib.BB_ERR_CAPACITY:
+                raise
+            print('\nLoading error model from {}'.format(filename), file=output)
+            sys.exit('Error: could not align the error model alternatives')   # the slot pool's limit, as _build_tables
+        finally:
+            data.close()
+        if any(info['fallback'] for info in infos):
+            return None
+        model.type = 'model'
+        model.kmer_size = infos[0]['k']
+        model.info = infos[0]
+        model._engine = engines[0]
+        model._host_tables = None
+        model._alternatives = model._probabilities = None
+        model._kmers, model._probs_loaded = [], []
+        print('\nLoading error model from {}'.format(filename), file=output)
+        print(f'\r  done: loaded error distributions for {model.info["n_rows"]} {model.kmer_size}-mers', file=output)
+        return model
+
+    @property
+    def _tables(self):
+        if self._host_tables is None:
+            self._host_tables = self._engine.download_error_model(self.info)
+        return self._host_tables
+
+    @_tables.setter
+    def _tables(self, tables):
+        self._host_tables = tables
+
+
+def load_error_model(name, engines, output=sys.stderr):
+    """ErrorModel(name) for the engines that simulate with it: a model file is built on their GPUs (DeviceErrorModel);
+    'random', the built-in models and a file off the device loader's fast path load as ErrorModel loads them."""
+    if name != 'random' and name not in BUILTIN_MODELS:
+        model = DeviceErrorModel.load(name, engines, output)
+        if model is not None:
+            return model
+    return ErrorModel(name, output)
+
+
 def add_one_random_change(kmer):
     """error_model.py:163-176."""
     result = [x for x in kmer]

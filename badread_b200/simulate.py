@@ -28,7 +28,7 @@ import numpy as np
 
 from . import settings
 from .engine import Engine, FastaFile, FragmentBatch, default_engine, next_read_index, run_each
-from .error_model import ErrorModel
+from .error_model import ErrorModel, load_error_model
 from .fragment_lengths import FragmentLengths
 from .identities import Identities
 from .misc import float_to_str, load_fasta, load_fasta_arrays, str_is_int
@@ -470,7 +470,7 @@ def _simulate(args, output, stdout, seed, setup_rng, setup_nrng, engines):
     frag_lengths = FragmentLengths(args.mean_frag_length, args.frag_length_stdev, output)
     adjust_depths(ref, frag_lengths, args, setup_nrng)
     identities = Identities(args.mean_identity, args.identity_stdev, args.max_identity, output)
-    error_model = ErrorModel(args.error_model, output)
+    error_model = load_error_model(args.error_model, engines, output)
     qscore_model = QScoreModel(args.qscore_model, output)
     print_glitch_summary(args.glitch_rate, args.glitch_size, args.glitch_skip, output)
     random_start, random_end = build_random_adapters(args, setup_rng)

@@ -126,6 +126,44 @@ BB_API int bb_upload_error_model_kmers(bb_ctx *ctx, int k, int32_t n_rows, const
                                 const double *cum, const uint8_t *flags, const uint32_t *slots, const uint8_t *pool,
                                 int64_t pool_len);
 
+/* Why bb_load_error_model_file left a model file to the host loader (bits of bb_em_load_info.fallback). */
+enum bb_em_fallback {
+    BB_EM_FALLBACK_NUMBER = 1,        /* a probability off the fast path: exponent, sign, inf/nan, >= 2^53, > 22 decimals */
+    BB_EM_FALLBACK_DUPLICATE = 2,     /* two lines have the same k-mer */
+    BB_EM_FALLBACK_K = 4,             /* a k-mer whose length is not the first line's, or k outside 3..16 */
+    BB_EM_FALLBACK_BASE = 8,          /* a byte other than ACGT in a k-mer or an alternative */
+    BB_EM_FALLBACK_SYNTAX = 16,       /* a stray ';' or ',', a missing probability, ... */
+    BB_EM_FALLBACK_CR = 32,           /* a '\r' (text-mode line ends) */
+    BB_EM_FALLBACK_LONG_ALT = 64,     /* an alternative longer than 64 bases */
+    BB_EM_FALLBACK_ALT_ENDS = 128,    /* an alternative shorter than 2 bases or not keeping the k-mer's first and last base */
+    BB_EM_FALLBACK_EMPTY_LINE = 256,  /* an empty line, or an empty file */
+    BB_EM_FALLBACK_INPUT = 512,       /* a gzip stream that does not inflate, or a bzip2 / zip file */
+    BB_EM_FALLBACK_SIZE = 1024        /* more than 2^31 - 1 rows or entries */
+};
+
+typedef struct bb_em_load_info {
+    int32_t k;
+    int32_t index;          /* 1: dense kmer_to_row[4^k], 2: hash table of the rows' k-mers */
+    int64_t n_rows, n_entries, n_alts, pool_bytes;
+    int64_t text_bytes;     /* the model text (inflated) */
+    uint32_t fallback;      /* bb_em_fallback bits; 0 when the tables were built and installed */
+    int32_t reserved;
+    double ms_inflate, ms_parse, ms_align, ms_tables, ms_index, ms_total;   /* host clock, each stage synchronised */
+} bb_em_load_info;
+
+/* An error model file's bytes (plain text, gzip or BGZF; page-locked memory copies fastest) turned into the tables of
+ *  ErrorModel(file) on the context's GPU and installed as bb_upload_error_model(_kmers) would install them: the dense
+ *  index for k <= 12, else the hash table.  A file off the loader's fast path sets info->fallback and installs nothing
+ *  (the model in use stays); the caller then loads it with the host loader.  BB_ERR_CAPACITY when the slot pool outgrows
+ *  2^24 bytes, as the host loader refuses it. */
+BB_API int bb_load_error_model_file(bb_ctx *ctx, const uint8_t *bytes, int64_t n, bb_em_load_info *info);
+
+/* The tables installed by the last bb_load_error_model_file, copied to host arrays sized by its info: kmer_to_row[4^k]
+ *  (dense index only), kmer_codes[n_rows], row_off[n_rows + 1], cum / probs / flags[n_entries], slots[n_entries * k],
+ *  pool[max(pool_bytes, 1)].  NULL skips an array.  BB_ERR_STATE when the installed model came from another call. */
+BB_API int bb_download_error_model(bb_ctx *ctx, int32_t *kmer_to_row, int64_t *kmer_codes, int32_t *row_off, double *cum,
+                                   double *probs, uint8_t *flags, uint32_t *slots, uint8_t *pool);
+
 /* Qscore model tables (flat form of QScoreModel.scores / .probabilities, qscore_model.py:178-271).
  *  Key i is the CIGAR string key_chars[key_off[i] .. key_off[i+1]) over {=,X,I,D}, of any length;
  *  row_off[n_keys+1]; scores / cum per entry. kmer_size as QScoreModel.kmer_size.  A repeated key keeps its last row
