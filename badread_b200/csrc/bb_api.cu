@@ -15,30 +15,11 @@
 #include <thread>
 #include <vector>
 
+#include "bb_call.h"
 #include "bb_kernels.cuh"
 #include "bb_launch.h"
 
 namespace {
-
-struct DevBuf {  // grow-only device allocation, freed with its owner
-    void *p = nullptr;
-    size_t cap = 0;
-    DevBuf() = default;
-    DevBuf(const DevBuf &) = delete;
-    DevBuf &operator=(const DevBuf &) = delete;  // (so a Worker or a context cannot be copied either)
-    DevBuf(DevBuf &&o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
-    ~DevBuf() { release(); }
-    cudaError_t ensure(size_t bytes) {
-        if (bytes <= cap) return cudaSuccess;
-        release();
-        size_t want = bytes + bytes / 8 + 256;
-        cudaError_t e = cudaMalloc(&p, want);
-        if (e == cudaSuccess) cap = want;
-        return e;
-    }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
-    template <typename T> T *as() const { return reinterpret_cast<T *>(p); }
-};
 
 constexpr int BB_MAX_ROUNDS = 15;  // error-loop rounds a run can enqueue (16 counters each, see BB_ROUND_BASE)
 // per-level snapshot of the queue counters (bb_last_run_work): [pipeline][level < BB_MAX_LEVELS][the BBQ_NODE_CLASSES
@@ -442,15 +423,6 @@ extern "C" int bb_download_reference(bb_ctx *ctx, int64_t offset, int64_t n, uin
 }
 
 // ---- the reference from a FASTA file parsed on the device (bb_fasta.cuh)
-// Exactly `bytes` (at least 1) in buf: the loader's buffers are the size of the reference, so no slack.
-static cudaError_t alloc_exact(DevBuf &buf, size_t bytes) {
-    buf.release();
-    bytes = std::max<size_t>(bytes, 1);
-    cudaError_t e = cudaMalloc(&buf.p, bytes);
-    if (e == cudaSuccess) buf.cap = bytes;
-    return e;
-}
-
 static void fasta_reset(bb_ctx *ctx) {
     ctx->fa_kept.release();
     ctx->fa_n_kept = -1;
@@ -470,58 +442,34 @@ extern "C" int bb_fasta_parse(bb_ctx *ctx, const uint8_t *data, int64_t n, int i
     ctx->ref.release();   // (replaced by bb_fasta_reference; freed first, so that the parse has its memory)
     ctx->ref_len = 0;
     const cudaStream_t st = ctx->w0().stream;
-    DevBuf text, scratch, hdr, idx, htext;
-    int64_t len = n;
-    if (is_bgzf) {
-        uint8_t *p = nullptr;
-        char msg[256];
-        if (const int rc = bbl_gzip_inflate_device(st, data, n, 0, &p, &len, &ctx->gz_stats, msg, sizeof(msg)))
-            return set_err(ctx, rc, msg);
-        text.p = p;
-        text.cap = (size_t)std::max<int64_t>(len, 16);
-    } else {
-        BB_CUDA(ctx, alloc_exact(text, (size_t)n));
-        if (n) BB_CUDA(ctx, cudaMemcpyAsync(text.p, data, (size_t)n, cudaMemcpyHostToDevice, st));
-    }
-    BB_CUDA(ctx, alloc_exact(scratch, bbl_fasta_scratch_bytes(len)));
-    bbl_fasta_scan(st, text.as<uint8_t>(), len, scratch.p);
-    int64_t totals[2] = {0, 0};
-    BB_CUDA(ctx, cudaMemcpyAsync(totals, bbl_fasta_totals(scratch.p, len), sizeof(totals), cudaMemcpyDeviceToHost, st));
-    BB_CUDA(ctx, cudaStreamSynchronize(st));
-    const int64_t kept = totals[0], nh = totals[1];
-    if (nh > INT32_MAX) return set_err(ctx, BB_ERR_ARG, "bb_fasta_parse: more than 2^31 - 1 header lines");
-    BB_CUDA(ctx, alloc_exact(ctx->fa_kept, (size_t)kept));
-    BB_CUDA(ctx, alloc_exact(hdr, 3 * sizeof(int64_t) * (size_t)nh));
-    int64_t *d_start = hdr.as<int64_t>(), *d_end = d_start + nh, *d_kept = d_end + nh;
-    bbl_fasta_emit(st, text.as<uint8_t>(), len, scratch.p, ctx->fa_kept.as<uint8_t>(), d_start, d_end, d_kept);
-    BB_CUDA(ctx, cudaGetLastError());
-    std::vector<int64_t> h((size_t)(3 * nh));
-    if (nh) BB_CUDA(ctx, cudaMemcpyAsync(h.data(), hdr.p, h.size() * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    BB_CUDA(ctx, cudaStreamSynchronize(st));
-    // the header texts (after the '>', up to the newline) gathered into one buffer
-    std::vector<int64_t> lo_off((size_t)(2 * nh + 1));
-    lo_off[(size_t)nh] = 0;
-    for (int64_t k = 0; k < nh; k++) {
-        lo_off[(size_t)k] = h[(size_t)k] + 1;
-        lo_off[(size_t)(nh + k + 1)] = lo_off[(size_t)(nh + k)] + (h[(size_t)(nh + k)] - h[(size_t)k] - 1);
-    }
-    const int64_t tlen = lo_off[(size_t)(2 * nh)];
-    ctx->fa_text.resize((size_t)tlen);
-    if (tlen) {
-        if (const int rc = upload(ctx, st, idx, lo_off.data(), lo_off.size())) return rc;
-        BB_CUDA(ctx, alloc_exact(htext, (size_t)tlen));
-        bbl_fasta_gather(st, text.as<uint8_t>(), idx.as<int64_t>(), idx.as<int64_t>() + nh, (int32_t)nh, tlen, htext.as<uint8_t>());
+    return context_call(ctx->err, [&]() -> int {
+        Scratch S;
+        int64_t len = 0;
+        const DevBuf text = text_to_device(S, st, data, n, is_bgzf, &len, &ctx->gz_stats, "bb_fasta_parse: the FASTA text");
+        void *scratch = S.get<uint8_t>((int64_t)bbl_fasta_scratch_bytes(len), "bb_fasta_parse: scratch");
+        bbl_fasta_scan(st, text.as<uint8_t>(), len, scratch);
+        int64_t totals[2] = {0, 0};
+        d2h(totals, bbl_fasta_totals(scratch, len), 2, st);
+        const int64_t kept = totals[0], nh = totals[1];
+        if (nh > INT32_MAX) return set_err(ctx, BB_ERR_ARG, "bb_fasta_parse: more than 2^31 - 1 header lines");
+        BB_CUDA(ctx, ctx->fa_kept.alloc((size_t)kept));   // (the size of the reference: no slack)
+        int64_t *d_start = S.get<int64_t>(3 * nh, "bb_fasta_parse: the header lines"), *d_end = d_start + nh, *d_kept = d_end + nh;
+        bbl_fasta_emit(st, text.as<uint8_t>(), len, scratch, ctx->fa_kept.as<uint8_t>(), d_start, d_end, d_kept);
         BB_CUDA(ctx, cudaGetLastError());
-        BB_CUDA(ctx, cudaMemcpyAsync(&ctx->fa_text[0], htext.p, (size_t)tlen, cudaMemcpyDeviceToHost, st));
+        std::vector<int64_t> h((size_t)(3 * nh));
+        if (nh) BB_CUDA(ctx, cudaMemcpyAsync(h.data(), d_start, h.size() * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
         BB_CUDA(ctx, cudaStreamSynchronize(st));
-    }
-    ctx->fa_text_off.assign(lo_off.begin() + nh, lo_off.end());
-    ctx->fa_kept_off.assign(h.begin() + 2 * nh, h.end());
-    ctx->fa_n_kept = kept;
-    *n_headers = (int32_t)nh;
-    *text_bytes = tlen;
-    *n_kept = kept;
-    return BB_OK;
+        // the header texts: after the '>', up to the newline
+        std::vector<int64_t> lo(h.begin(), h.begin() + nh), hi(h.begin() + nh, h.begin() + 2 * nh);
+        for (int64_t &x : lo) x++;
+        ctx->fa_text_off = gather_spans(S, st, text.as<uint8_t>(), lo, hi, &ctx->fa_text, "bb_fasta_parse: the header texts");
+        ctx->fa_kept_off.assign(h.begin() + 2 * nh, h.end());
+        ctx->fa_n_kept = kept;
+        *n_headers = (int32_t)nh;
+        *text_bytes = (int64_t)ctx->fa_text.size();
+        *n_kept = kept;
+        return BB_OK;
+    });
 }
 
 extern "C" int bb_last_gzip_stats(const bb_ctx *ctx, bb_gzip_stats *stats) {
@@ -562,12 +510,10 @@ extern "C" int bb_fasta_reference(bb_ctx *ctx, int32_t n_contigs, const int64_t 
     BB_CUDA(ctx, cudaSetDevice(ctx->device));
     const cudaStream_t st = ctx->w0().stream;
     if (in_place) {
-        ctx->ref.release();
-        std::swap(ctx->ref.p, ctx->fa_kept.p);
-        std::swap(ctx->ref.cap, ctx->fa_kept.cap);
+        ctx->ref = std::move(ctx->fa_kept);
     } else {
         DevBuf idx;
-        BB_CUDA(ctx, alloc_exact(ctx->ref, (size_t)total));
+        BB_CUDA(ctx, ctx->ref.alloc((size_t)total));
         if (const int rc = upload(ctx, st, idx, lo_off.data(), lo_off.size())) return rc;
         bbl_fasta_gather(st, ctx->fa_kept.as<uint8_t>(), idx.as<int64_t>(), idx.as<int64_t>() + n_contigs, n_contigs, total,
                          ctx->ref.as<uint8_t>());
@@ -655,13 +601,6 @@ extern "C" int bb_upload_error_model_kmers(bb_ctx *ctx, int k, int32_t n_rows, c
     return BB_OK;
 }
 
-// Takes ownership of a device allocation
-static void adopt(DevBuf &buf, void *p, size_t bytes) {
-    buf.release();
-    buf.p = p;
-    buf.cap = bytes;
-}
-
 extern "C" int bb_load_error_model_file(bb_ctx *ctx, const uint8_t *bytes, int64_t n, bb_em_load_info *info) {
     if (!ctx || n < 0 || (n && !bytes) || !info) return set_err(ctx, BB_ERR_ARG, "bb_load_error_model_file: bad arguments");
     BB_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -676,82 +615,69 @@ extern "C" int bb_load_error_model_file(bb_ctx *ctx, const uint8_t *bytes, int64
         info->fallback = BB_EM_FALLBACK_INPUT;
         return BB_OK;
     }
-    DevBuf text;
-    int64_t len = n;
-    if (gz) {
-        uint8_t *p = nullptr;
-        char msg[256];
+    return context_call(ctx->err, [&]() -> int {
+        Scratch S;
+        int64_t len = 0;
         bb_gzip_stats stats{};
-        const int rc = bbl_gzip_inflate_device(st, bytes, n, 0, &p, &len, &stats, msg, sizeof(msg));
-        if (rc == BB_ERR_ARG) {   // not a stream gzip.open reads either: the host loader reports it
-            info->fallback = BB_EM_FALLBACK_INPUT;
+        DevBuf text;
+        try {
+            text = text_to_device(S, st, bytes, n, gz, &len, &stats, "bb_load_error_model_file: the file");
+        } catch (const Fail &f) {
+            if (f.rc != BB_ERR_ARG) throw;
+            info->fallback = BB_EM_FALLBACK_INPUT;   // not a stream gzip.open reads either: the host loader reports it
             return BB_OK;
         }
-        if (rc) return set_err(ctx, rc, msg);
-        text.p = p;
-        text.cap = (size_t)std::max<int64_t>(len, 16);
-    } else {
-        BB_CUDA(ctx, alloc_exact(text, (size_t)n));
-        if (n) BB_CUDA(ctx, cudaMemcpyAsync(text.p, bytes, (size_t)n, cudaMemcpyHostToDevice, st));
-        BB_CUDA(ctx, cudaStreamSynchronize(st));
-    }
-    auto t = std::chrono::steady_clock::now();
-    info->ms_inflate = std::chrono::duration<double, std::milli>(t - t0).count();
-    info->text_bytes = len;
-    BBEmLoadOut out;
-    char msg[256];
-    int rc = bbl_em_load(st, text.as<uint8_t>(), len, true, info, &out, msg, sizeof(msg));
-    text.release();
-    // the hash index for k > 12: BBEmHashTable's builder over the row codes made on the device
-    BBEmHashTable hash;
-    if (rc == BB_OK && !info->fallback && !out.kmer_to_row) {
-        std::vector<int64_t> codes((size_t)info->n_rows);
-        BB_CUDA(ctx, cudaMemcpy(codes.data(), out.codes, codes.size() * sizeof(int64_t), cudaMemcpyDeviceToHost));
-        std::string err;
-        if (!bb_build_em_hash(info->k, (int32_t)info->n_rows, codes.data(), hash, err)) info->fallback |= BB_EM_FALLBACK_DUPLICATE;
-    }
-    if (rc != BB_OK || info->fallback) {
-        bbl_em_load_free(&out);
-        return rc == BB_OK ? BB_OK : set_err(ctx, rc, msg);
-    }
-    ctx->have_em = false;
-    ctx->em = BBErrorModelDev{};
-    ctx->em_hash = BBEmHashDev{};
-    const size_t ne = (size_t)info->n_entries, nr = (size_t)info->n_rows;
-    if (out.kmer_to_row) {
-        adopt(ctx->em_k2r, out.kmer_to_row, ((size_t)1 << (2 * info->k)) * sizeof(int32_t));
-        info->index = 1;
-    } else {
-        if (const int urc = upload(ctx, st, ctx->em_hentries, hash.entries.data(), hash.entries.size())) {
-            bbl_em_load_free(&out);
-            return urc;
+        if (!gz) BB_CUDA(ctx, cudaStreamSynchronize(st));
+        auto t = std::chrono::steady_clock::now();
+        info->ms_inflate = std::chrono::duration<double, std::milli>(t - t0).count();
+        info->text_bytes = len;
+        BBEmLoadOut out;
+        bbl_em_load(st, text.as<uint8_t>(), len, true, info, &out);
+        text.release();
+        // the hash index for k > 12: BBEmHashTable's builder over the row codes made on the device
+        BBEmHashTable hash;
+        if (!info->fallback && !out.kmer_to_row.p) {
+            std::vector<int64_t> codes((size_t)info->n_rows);
+            BB_CUDA(ctx, cudaMemcpy(codes.data(), out.codes.p, codes.size() * sizeof(int64_t), cudaMemcpyDeviceToHost));
+            std::string err;
+            if (!bb_build_em_hash(info->k, (int32_t)info->n_rows, codes.data(), hash, err)) info->fallback |= BB_EM_FALLBACK_DUPLICATE;
         }
-        info->index = 2;
-    }
-    adopt(ctx->em_codes, out.codes, nr * sizeof(int64_t));
-    adopt(ctx->em_rowoff, out.row_off, (nr + 1) * sizeof(int32_t));
-    adopt(ctx->em_cum, out.cum, ne * sizeof(double));
-    adopt(ctx->em_probs, out.probs, ne * sizeof(double));
-    adopt(ctx->em_flags, out.flags, std::max<size_t>(ne, 1));
-    adopt(ctx->em_slots, out.slots, std::max<size_t>(ne * info->k, 1) * sizeof(uint32_t));
-    adopt(ctx->em_pool, out.pool, (size_t)std::max<int64_t>(info->pool_bytes, 1));
-    adopt(ctx->em_rowinfo, out.rowinfo, nr * sizeof(BBRowInfo));
-    BB_CUDA(ctx, cudaStreamSynchronize(st));
-    const auto t1 = std::chrono::steady_clock::now();
-    info->ms_index = std::chrono::duration<double, std::milli>(t1 - t).count() - info->ms_parse - info->ms_align - info->ms_tables;
-    info->ms_total = std::chrono::duration<double, std::milli>(t1 - t0).count();
-    ctx->em.k = info->k; ctx->em.type = 1;
-    ctx->em.kmer_to_row = info->index == 1 ? ctx->em_k2r.as<int32_t>() : nullptr;
-    ctx->em.row_off = ctx->em_rowoff.as<int32_t>();
-    ctx->em.cum = ctx->em_cum.as<double>(); ctx->em.flags = ctx->em_flags.as<uint8_t>();
-    ctx->em.slots = ctx->em_slots.as<uint32_t>(); ctx->em.pool = ctx->em_pool.as<uint8_t>();
-    ctx->em.rowinfo = ctx->em_rowinfo.as<BBRowInfo>();
-    if (info->index == 2) { ctx->em_hash.entries = ctx->em_hentries.as<unsigned long long>(); ctx->em_hash.bits = hash.bits; }
-    ctx->em_info = *info;
-    ctx->em_loaded = true;
-    ctx->have_em = true;
-    for (const auto &w : ctx->workers) w->uploaded = false;  // the fragment layout of a batch depends on k
-    return BB_OK;
+        if (info->fallback) return BB_OK;
+        ctx->have_em = false;
+        ctx->em = BBErrorModelDev{};
+        ctx->em_hash = BBEmHashDev{};
+        if (out.kmer_to_row.p) {
+            ctx->em_k2r = std::move(out.kmer_to_row);
+            info->index = 1;
+        } else {
+            if (const int urc = upload(ctx, st, ctx->em_hentries, hash.entries.data(), hash.entries.size())) return urc;
+            info->index = 2;
+        }
+        ctx->em_codes = std::move(out.codes);
+        ctx->em_rowoff = std::move(out.row_off);
+        ctx->em_cum = std::move(out.cum);
+        ctx->em_probs = std::move(out.probs);
+        ctx->em_flags = std::move(out.flags);
+        ctx->em_slots = std::move(out.slots);
+        ctx->em_pool = std::move(out.pool);
+        ctx->em_rowinfo = std::move(out.rowinfo);
+        BB_CUDA(ctx, cudaStreamSynchronize(st));
+        const auto t1 = std::chrono::steady_clock::now();
+        info->ms_index = std::chrono::duration<double, std::milli>(t1 - t).count() - info->ms_parse - info->ms_align - info->ms_tables;
+        info->ms_total = std::chrono::duration<double, std::milli>(t1 - t0).count();
+        ctx->em.k = info->k; ctx->em.type = 1;
+        ctx->em.kmer_to_row = info->index == 1 ? ctx->em_k2r.as<int32_t>() : nullptr;
+        ctx->em.row_off = ctx->em_rowoff.as<int32_t>();
+        ctx->em.cum = ctx->em_cum.as<double>(); ctx->em.flags = ctx->em_flags.as<uint8_t>();
+        ctx->em.slots = ctx->em_slots.as<uint32_t>(); ctx->em.pool = ctx->em_pool.as<uint8_t>();
+        ctx->em.rowinfo = ctx->em_rowinfo.as<BBRowInfo>();
+        if (info->index == 2) { ctx->em_hash.entries = ctx->em_hentries.as<unsigned long long>(); ctx->em_hash.bits = hash.bits; }
+        ctx->em_info = *info;
+        ctx->em_loaded = true;
+        ctx->have_em = true;
+        for (const auto &w : ctx->workers) w->uploaded = false;  // the fragment layout of a batch depends on k
+        return BB_OK;
+    });
 }
 
 extern "C" int bb_download_error_model(bb_ctx *ctx, int32_t *kmer_to_row, int64_t *kmer_codes, int32_t *row_off, double *cum,

@@ -5,23 +5,20 @@
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <unordered_map>
 #include <vector>
 
 #include "../../include/badread_b200.h"
 
-void bbm_set_error(const char *msg);   // bb_tu_models.cu
+#include "bb_call.h"
 
 namespace {
 
 // BAM's CIGAR op codes (SAM specification §4.2.2): M I D N S H P = X
 constexpr char kOps[] = "MIDNSHP=X";
 enum { OP_M = 0, OP_I = 1, OP_D = 2, OP_N = 3, OP_S = 4, OP_H = 5, OP_P = 6, OP_EQ = 7, OP_X = 8 };
-
-struct Fail {   // thrown with the message bb_model_error() reports
-    std::string msg;
-};
 
 }  // namespace
 
@@ -65,9 +62,9 @@ struct bb_aln_set {
         for (int64_t i = c0; i < c1; i++) {
             const uint32_t op = cigar[i] & 15u, n = cigar[i] >> 4;
             if (op == OP_N || op == OP_P)
-                throw Fail{"Error: the CIGAR of read " + name + " has an " + kOps[op] +
+                throw Fail{BB_ERR_ARG, "Error: the CIGAR of read " + name + " has an " + kOps[op] +
                            " operation (skipped regions and padding are not supported)"};
-            if (op > OP_X) throw Fail{"Error: invalid CIGAR operation in the record of read " + name};
+            if (op > OP_X) throw Fail{BB_ERR_ARG, "Error: invalid CIGAR operation in the record of read " + name};
             const bool clip = op == OP_S || op == OP_H;
             hard |= op == OP_H;
             if (op != OP_D) rlen += n;
@@ -81,7 +78,7 @@ struct bb_aln_set {
                 cols += n;
             }
         }
-        if (!has_as) throw Fail{"Error: no alignment score"};
+        if (!has_as) throw Fail{BB_ERR_ARG, "Error: no alignment score"};
         const bool reverse = (fl & 16) != 0;
         read_id.push_back(read(name.data(), name.size()));
         ref_id.push_back(rid);
@@ -147,18 +144,18 @@ void parse_sam(bb_aln_set &S, const char *text, int64_t n, int64_t max_records) 
         if (f.size() < 11 || !parse_int(f[1].first, f[1].second, &fl) || !parse_int(f[3].first, f[3].second, &pos)) {
             char msg[128];
             std::snprintf(msg, sizeof(msg), "Error: line %lld of the alignment file is not a SAM record", (long long)line_no);
-            throw Fail{msg};
+            throw Fail{BB_ERR_ARG, msg};
         }
         const std::string rname(f[2].first, f[2].second);
         if ((fl & 4) || rname == "*") continue;
         const std::string name(f[0].first, f[0].second);
-        if (f[5].second - f[5].first == 1 && *f[5].first == '*') throw Fail{"Error: no CIGAR string found"};
+        if (f[5].second - f[5].first == 1 && *f[5].first == '*') throw Fail{BB_ERR_ARG, "Error: no CIGAR string found"};
         for (const char *c = f[5].first; c < f[5].second;) {
             int64_t len = 0;
             const char *d = c;
             while (d < f[5].second && *d >= '0' && *d <= '9' && len < ((int64_t)1 << 28)) len = len * 10 + (*d++ - '0');
             const char *op = d < f[5].second ? std::strchr(kOps, *d) : nullptr;
-            if (d == c || !op || !*d) throw Fail{"Error: invalid CIGAR string in the record of read " + name};
+            if (d == c || !op || !*d) throw Fail{BB_ERR_ARG, "Error: invalid CIGAR string in the record of read " + name};
             S.cigar.push_back(((uint32_t)len << 4) | (uint32_t)(op - kOps));
             c = d + 1;
         }
@@ -186,23 +183,23 @@ void parse_sam(bb_aln_set &S, const char *text, int64_t n, int64_t max_records) 
 
 void parse_bam(bb_aln_set &S, const uint8_t *d, int64_t n, int64_t max_records) {
     auto need = [&](int64_t at, int64_t len, const char *what) {
-        if (at < 0 || len < 0 || at + len > n) throw Fail{std::string("Error: the BAM file is truncated (") + what + ")"};
+        if (at < 0 || len < 0 || at + len > n) throw Fail{BB_ERR_ARG, std::string("Error: the BAM file is truncated (") + what + ")"};
     };
     auto i32 = [&](int64_t at) { int32_t v; std::memcpy(&v, d + at, 4); return v; };
     auto u16 = [&](int64_t at) { uint16_t v; std::memcpy(&v, d + at, 2); return v; };
     need(0, 12, "header");
-    if (std::memcmp(d, "BAM\1", 4) != 0) throw Fail{"Error: the alignment file is not BAM (no BAM magic after inflating)"};
+    if (std::memcmp(d, "BAM\1", 4) != 0) throw Fail{BB_ERR_ARG, "Error: the alignment file is not BAM (no BAM magic after inflating)"};
     int64_t at = 8 + (int64_t)i32(4);
     need(at, 4, "header");
     const int32_t n_ref = i32(at);
     at += 4;
-    if (n_ref < 0) throw Fail{"Error: the BAM header is invalid (negative reference count)"};
+    if (n_ref < 0) throw Fail{BB_ERR_ARG, "Error: the BAM header is invalid (negative reference count)"};
     for (int32_t r = 0; r < n_ref; r++) {
         need(at, 4, "reference names");
         const int32_t l_name = i32(at);
         need(at + 4, (int64_t)l_name + 4, "reference names");
-        if (l_name < 1) throw Fail{"Error: the BAM header is invalid (empty reference name)"};
-        if (S.ref((const char *)d + at + 4, (size_t)l_name - 1) != r) throw Fail{"Error: the BAM header names a reference twice"};
+        if (l_name < 1) throw Fail{BB_ERR_ARG, "Error: the BAM header is invalid (empty reference name)"};
+        if (S.ref((const char *)d + at + 4, (size_t)l_name - 1) != r) throw Fail{BB_ERR_ARG, "Error: the BAM header names a reference twice"};
         at += 4 + (int64_t)l_name + 4;
     }
     int64_t n_rec = 0;
@@ -211,7 +208,7 @@ void parse_bam(bb_aln_set &S, const uint8_t *d, int64_t n, int64_t max_records) 
         need(at, 4, "record");
         const int64_t bs = i32(at), r0 = at + 4, r1 = r0 + bs;
         need(r0, bs, "record");
-        if (bs < 32) throw Fail{"Error: the BAM file holds an invalid record"};
+        if (bs < 32) throw Fail{BB_ERR_ARG, "Error: the BAM file holds an invalid record"};
         at = r1;
         const int32_t ref_id = i32(r0), pos = i32(r0 + 4);
         const int l_name = d[r0 + 8];
@@ -219,11 +216,11 @@ void parse_bam(bb_aln_set &S, const uint8_t *d, int64_t n, int64_t max_records) 
         const int32_t l_seq = i32(r0 + 16);
         const int64_t p_name = r0 + 32, p_cig = p_name + l_name, p_seq = p_cig + 4 * (int64_t)n_cig;
         const int64_t p_qual = p_seq + ((int64_t)l_seq + 1) / 2, p_tags = p_qual + l_seq;
-        if (l_name < 1 || l_seq < 0 || p_tags > r1) throw Fail{"Error: the BAM file holds an invalid record"};
+        if (l_name < 1 || l_seq < 0 || p_tags > r1) throw Fail{BB_ERR_ARG, "Error: the BAM file holds an invalid record"};
         if ((fl & 4) || ref_id < 0) continue;
-        if (ref_id >= n_ref) throw Fail{"Error: a BAM record names a reference the header does not list"};
+        if (ref_id >= n_ref) throw Fail{BB_ERR_ARG, "Error: a BAM record names a reference the header does not list"};
         const std::string name((const char *)d + p_name, (size_t)l_name - 1);
-        if (n_cig == 0) throw Fail{"Error: no CIGAR string found"};
+        if (n_cig == 0) throw Fail{BB_ERR_ARG, "Error: no CIGAR string found"};
         for (int k = 0; k < n_cig; k++) {
             uint32_t c;
             std::memcpy(&c, d + p_cig + 4 * k, 4);
@@ -238,7 +235,7 @@ void parse_bam(bb_aln_set &S, const uint8_t *d, int64_t n, int64_t max_records) 
         int64_t as = 0, nm = 0;
         for (int64_t t = p_tags; t < r1;) {
             need(t, 3, "tags");
-            if (t + 3 > r1) throw Fail{"Error: the BAM file holds an invalid record"};
+            if (t + 3 > r1) throw Fail{BB_ERR_ARG, "Error: the BAM file holds an invalid record"};
             const char a = (char)d[t], b = (char)d[t + 1], type = (char)d[t + 2];
             int64_t v = 0, size;
             t += 3;
@@ -248,20 +245,20 @@ void parse_bam(bb_aln_set &S, const uint8_t *d, int64_t n, int64_t max_records) 
                 case 'i': case 'I': case 'f': size = 4; break;
                 case 'Z': case 'H': {
                     const void *z = t < r1 ? std::memchr(d + t, 0, (size_t)(r1 - t)) : nullptr;
-                    if (!z) throw Fail{"Error: the BAM file holds an invalid record"};
+                    if (!z) throw Fail{BB_ERR_ARG, "Error: the BAM file holds an invalid record"};
                     size = (const uint8_t *)z - (d + t) + 1;
                     break;
                 }
                 case 'B': {
-                    if (t + 5 > r1) throw Fail{"Error: the BAM file holds an invalid record"};
+                    if (t + 5 > r1) throw Fail{BB_ERR_ARG, "Error: the BAM file holds an invalid record"};
                     const char sub = (char)d[t];
                     const int64_t w = sub == 'c' || sub == 'C' ? 1 : sub == 's' || sub == 'S' ? 2 : 4;
                     size = 5 + w * (int64_t)(uint32_t)i32(t + 1);
                     break;
                 }
-                default: throw Fail{"Error: the BAM file holds an invalid record"};
+                default: throw Fail{BB_ERR_ARG, "Error: the BAM file holds an invalid record"};
             }
-            if (t + size > r1) throw Fail{"Error: the BAM file holds an invalid record"};
+            if (t + size > r1) throw Fail{BB_ERR_ARG, "Error: the BAM file holds an invalid record"};
             const bool integer = type == 'c' || type == 'C' || type == 's' || type == 'S' || type == 'i' || type == 'I';
             if (integer) {
                 switch (type) {
@@ -304,7 +301,7 @@ void parse_paf(bb_aln_set &S, const char *text, int64_t n, int64_t max_records) 
             if (!tab) break;
             c = tab + 1;
         }
-        if (f.size() < 11) throw Fail{"Error: alignment file does not seem to be in PAF format"};
+        if (f.size() < 11) throw Fail{BB_ERR_ARG, "Error: alignment file does not seem to be in PAF format"};
         // int() of a field: surrounding whitespace, an optional sign, decimal digits
         auto num = [&](const char *a, const char *b, int64_t lo, int64_t hi, const char *what) {
             while (a < b && paf_space(*a)) a++;
@@ -314,7 +311,7 @@ void parse_paf(bb_aln_set &S, const char *text, int64_t n, int64_t max_records) 
                 char msg[160];
                 std::snprintf(msg, sizeof(msg), "Error: %s on line %lld of the alignment file is not an integer in [%lld, %lld]",
                               what, (long long)line_no, (long long)lo, (long long)hi);
-                throw Fail{msg};
+                throw Fail{BB_ERR_ARG, msg};
             }
             return v;
         };
@@ -328,12 +325,12 @@ void parse_paf(bb_aln_set &S, const char *text, int64_t n, int64_t max_records) 
         if (cols == 0) {
             char msg[128];
             std::snprintf(msg, sizeof(msg), "Error: line %lld of the alignment file has 0 alignment columns (column 11)", (long long)line_no);
-            throw Fail{msg};
+            throw Fail{BB_ERR_ARG, msg};
         }
         if (cols - matching < INT32_MIN || cols - matching > INT32_MAX) {
             char msg[128];
             std::snprintf(msg, sizeof(msg), "Error: columns 10 and 11 on line %lld of the alignment file are out of range", (long long)line_no);
-            throw Fail{msg};
+            throw Fail{BB_ERR_ARG, msg};
         }
         const char *cg = nullptr, *cg_end = nullptr;
         bool has_as = false;
@@ -345,8 +342,8 @@ void parse_paf(bb_aln_set &S, const char *text, int64_t n, int64_t max_records) 
                 has_as = true;
             }
         }
-        if (!cg) throw Fail{"Error: no CIGAR string found"};
-        if (!has_as) throw Fail{"Error: no alignment score"};
+        if (!cg) throw Fail{BB_ERR_ARG, "Error: no CIGAR string found"};
+        if (!has_as) throw Fail{BB_ERR_ARG, "Error: no alignment score"};
         const std::string name(f[0].first, f[0].second);
         for (const char *c = cg; c < cg_end;) {   // re.findall(r'(\d+)([A-Za-z=])')
             if (*c < '0' || *c > '9') { c++; continue; }
@@ -357,7 +354,7 @@ void parse_paf(bb_aln_set &S, const char *text, int64_t n, int64_t max_records) 
             const uint32_t code = *d == 'M' ? OP_M : *d == 'I' ? OP_I : *d == 'D' ? OP_D : 15u;
             int64_t len = 0;
             for (const char *x = c; x < d && len < ((int64_t)1 << 28); x++) len = len * 10 + (*x - '0');
-            if (code != 15u && len >= ((int64_t)1 << 28)) throw Fail{"Error: a CIGAR run of read " + name + " is longer than 2^28 - 1"};
+            if (code != 15u && len >= ((int64_t)1 << 28)) throw Fail{BB_ERR_ARG, "Error: a CIGAR run of read " + name + " is longer than 2^28 - 1"};
             S.cigar.push_back(((uint32_t)(code == 15u ? 0 : len) << 4) | code);
             c = d + 1;
         }
@@ -384,24 +381,16 @@ void parse_paf(bb_aln_set &S, const char *text, int64_t n, int64_t max_records) 
 }  // namespace
 
 extern "C" int bb_aln_parse(const uint8_t *data, int64_t n, int is_bam, int64_t max_records, bb_aln_set **set) {
-    bbm_set_error("");
-    if (!set || n < 0 || (n > 0 && !data)) {
-        bbm_set_error("bb_aln_parse: invalid argument");
-        return BB_ERR_ARG;
-    }
+    if (!set || n < 0 || (n > 0 && !data)) return bad_argument("bb_aln_parse");
     *set = nullptr;
-    bb_aln_set *S = new bb_aln_set();
-    try {
+    return model_call([&] {
+        std::unique_ptr<bb_aln_set> S(new bb_aln_set());
         if (is_bam == BB_ALN_PAF) parse_paf(*S, (const char *)data, n, max_records);
         else if (is_bam) parse_bam(*S, data, n, max_records);
         else parse_sam(*S, (const char *)data, n, max_records);
-    } catch (const Fail &f) {
-        bbm_set_error(f.msg.c_str());
-        delete S;
-        return BB_ERR_ARG;
-    }
-    *set = S;
-    return BB_OK;
+        *set = S.release();
+        return BB_OK;
+    });
 }
 
 extern "C" int bb_aln_view_get(const bb_aln_set *S, bb_aln_view *v) {

@@ -1,7 +1,8 @@
 // bb_launch.h — host-side launchers of the heavy kernels.  Every kernel is a template (bb_kernels.cuh), so it is
 // compiled only by the translation unit that launches it: the heavy ones live in bb_tu_*.cu, one file each, and
 // build in parallel (the wide wavefront instantiations take minutes of ptxas each); bb_api.cu launches the light
-// ones itself.  All launchers are asynchronous on `st`; errors surface through cudaGetLastError() in the caller.
+// ones itself.  All launchers are asynchronous on `st`; errors surface through cudaGetLastError() in the caller.  The
+// input paths' helpers that the light units call too are declared in bb_call.h.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -62,33 +63,3 @@ void bbl_fasta_scan(cudaStream_t st, const uint8_t *text, int64_t n, void *scrat
 const int64_t *bbl_fasta_totals(const void *scratch, int64_t n);
 void bbl_fasta_emit(cudaStream_t st, const uint8_t *text, int64_t n, const void *scratch, uint8_t *kept, int64_t *hdr_start,
                     int64_t *hdr_end, int64_t *hdr_kept);
-// bb_c_comp's table (misc._COMP_TABLE) into table[256], for every unit that complements on the device
-void bbl_comp_table(uint8_t *table);
-// dst[dst_off[r] .. dst_off[r + 1]) = src[src_lo[r] ..] for r < n_ranges; total = dst_off[n_ranges] (device arrays)
-void bbl_fasta_gather(cudaStream_t st, const uint8_t *src, const int64_t *src_lo, const int64_t *dst_off, int32_t n_ranges,
-                      int64_t total, uint8_t *dst);
-// BGZF in host memory in[0..n) inflated on `st` into a new device allocation *out of *total bytes (cudaFree it): the
-// input goes through a device buffer of its own, released before the call returns.  BB_ERR_ARG with msg naming the member
-// (index and offset) for input that is not BGZF or a corrupt member, as bb_bgzf_decompress; BB_ERR_CUDA otherwise.
-int bbl_bgzf_inflate_device(cudaStream_t st, const uint8_t *in, int64_t n, uint8_t **out, int64_t *total, char *msg,
-                            size_t msg_len);
-// Any gzip stream in host memory in[0..n) inflated the same way (bb_tu_gunzip.cu): through bbl_bgzf_inflate_device when
-// every member is BGZF, else in chunks of chunk_bytes (0: the default); *stats as bb_gzip_decompress reports them.
-struct bb_gzip_stats;
-// An error model file's text[0..n) in device memory to its tables (bb_em_load.cuh), in new device allocations that
-// bbl_em_load_free releases.  kmer_to_row[4^k] only when `dense` and k <= 12.  info->fallback set: nothing to install.
-struct BBEmLoadOut {
-    int32_t *kmer_to_row = nullptr;
-    int64_t *codes = nullptr;
-    int32_t *row_off = nullptr;
-    double *cum = nullptr, *probs = nullptr;
-    uint8_t *flags = nullptr;
-    uint32_t *slots = nullptr;
-    uint8_t *pool = nullptr;
-    BBRowInfo *rowinfo = nullptr;
-};
-int bbl_em_load(cudaStream_t st, const uint8_t *text, int64_t n, bool dense, bb_em_load_info *info, BBEmLoadOut *out,
-                char *msg, size_t msg_len);
-void bbl_em_load_free(BBEmLoadOut *out);
-int bbl_gzip_inflate_device(cudaStream_t st, const uint8_t *in, int64_t n, int64_t chunk_bytes, uint8_t **out,
-                            int64_t *total, bb_gzip_stats *stats, char *msg, size_t msg_len);

@@ -1,4 +1,5 @@
 // bb_tu_fasta.cu — compiles the FASTA parser (bb_fasta.cuh) and enqueues its passes.
+#include "bb_call.h"
 #include "bb_fasta.cuh"
 #include "bb_launch.h"
 

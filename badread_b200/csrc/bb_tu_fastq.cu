@@ -5,7 +5,6 @@
 #include <cuda_runtime.h>
 
 #include <cstdint>
-#include <cstdio>
 #include <memory>
 #include <string>
 #include <string_view>
@@ -14,96 +13,31 @@
 
 #include "../../include/badread_b200.h"
 
+#include "bb_call.h"
 #include "bb_fastq.cuh"
-
-void bbm_set_error(const char *msg);   // bb_tu_models.cu
-int bbl_gzip_inflate_device(cudaStream_t st, const uint8_t *in, int64_t n, int64_t chunk_bytes, uint8_t **out,
-                            int64_t *total, bb_gzip_stats *stats, char *msg, size_t msg_len);   // (bb_launch.h)
-void bbl_comp_table(uint8_t *table);                                                      // (bb_launch.h)
-void bbl_fasta_gather(cudaStream_t st, const uint8_t *src, const int64_t *src_lo, const int64_t *dst_off, int32_t n_ranges,
-                      int64_t total, uint8_t *dst);                                          // (bb_launch.h)
 
 struct bb_fastq_set {
     int device = 0;
-    uint8_t *text = nullptr;      // the (inflated) file, until bb_flat_build has gathered from it
-    FastqRec *recs = nullptr;
+    DevBuf text;                  // the (inflated) file, until bb_flat_build has gathered from it
+    DevBuf recs;                  // FastqRec[n_rec]
     int64_t n_text = 0, n_rec = 0;
-    std::vector<char> names;      // record r's name: names[name_off[r] .. name_off[r + 1])
+    std::string names;            // record r's name: names[name_off[r] .. name_off[r + 1])
     std::vector<int64_t> name_off;
-    void release() {
-        cudaFree(text);
-        cudaFree(recs);
-        text = nullptr;
-        recs = nullptr;
-    }
-    ~bb_fastq_set() { release(); }
 };
 
 struct bb_flat_set {
     int32_t n = 0;
-    uint8_t *read = nullptr, *qual = nullptr, *ref = nullptr;
-    uint32_t *ops = nullptr;
-    int32_t *op_read0 = nullptr, *op_ref0 = nullptr;
+    DevBuf read, qual, ref, ops, op_read0, op_ref0;
     std::vector<int64_t> read_off{0}, ref_off{0}, ops_off{0};
-    ~bb_flat_set() {
-        for (void *p : {(void *)read, (void *)qual, (void *)ref, (void *)ops, (void *)op_read0, (void *)op_ref0}) cudaFree(p);
-    }
 };
 
 namespace {
 
-struct Fail {   // thrown with the return code and the message bb_model_error() reports
-    int rc;
-    std::string msg;
-};
-
-void check(cudaError_t e, const char *what) {
-    if (e != cudaSuccess) throw Fail{BB_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(e)};
-}
-
-// `count` elements of device memory (at least 16 bytes, not initialized: every kernel writes what it reads), for `stage`
-template <class X>
-X *dalloc(int64_t count, const char *stage) {
-    const size_t bytes = count * sizeof(X) > 16 ? (size_t)count * sizeof(X) : 16;
-    void *p = nullptr;
-    const cudaError_t e = cudaMalloc(&p, bytes);
-    if (e == cudaErrorMemoryAllocation) {
-        (void)cudaGetLastError();
-        throw Fail{BB_ERR_CAPACITY, std::string("Error: not enough device memory for ") + stage + " (" + std::to_string(bytes) +
-                                        " bytes asked for)"};
-    }
-    check(e, "cudaMalloc");
-    return (X *)p;
-}
-
-struct Scratch {   // what a call allocates for itself, released on every exit path
-    std::vector<void *> p;
-    ~Scratch() { for (void *q : p) cudaFree(q); }
-    template <class X>
-    X *get(int64_t count, const char *stage) {
-        X *q = dalloc<X>(count, stage);
-        p.push_back(q);
-        return q;
-    }
-};
-
-template <class X>
-void d2h(X *dst, const void *src, int64_t count) {
-    if (count > 0) check(cudaMemcpy(dst, src, (size_t)count * sizeof(X), cudaMemcpyDeviceToHost), "cudaMemcpy");
-}
-
-template <class X>
-X *upload(Scratch &S, const X *src, int64_t count, const char *stage) {
-    X *d = S.get<X>(count, stage);
-    if (count > 0) check(cudaMemcpy(d, src, (size_t)count * sizeof(X), cudaMemcpyHostToDevice), "cudaMemcpy");
-    return d;
-}
-
 unsigned grid(int64_t items, int64_t per) { return (unsigned)((items + per - 1) / per); }
 
 void parse(bb_fastq_set &F) {
-    Scratch S;
-    const uint8_t *text = F.text;
+    Scratch S(BB_ERR_CAPACITY);
+    const uint8_t *text = F.text.as<uint8_t>();
     const int64_t n = F.n_text, n_tiles = (n + FQ_TILE - 1) / FQ_TILE;
     // 1. the newlines
     int64_t *counts = S.get<int64_t>(n_tiles + 1, "the newline scan");
@@ -130,35 +64,26 @@ void parse(bb_fastq_set &F) {
     int64_t *rec_line = S.get<int64_t>(n_rec, "the record table");
     if (n_lt) fq_k_records<<<(unsigned)n_lt, FQ_THREADS>>>(text, nl, n_nl, n, n_lines, FQ_LINES_PER_THREAD, state, base, rec_line);
     // 3. the spans
-    F.recs = dalloc<FastqRec>(n_rec, "the record table");
+    F.recs = S.result((size_t)n_rec * sizeof(FastqRec), "the record table");
     F.n_rec = n_rec;
+    FastqRec *recs = F.recs.as<FastqRec>();
     unsigned long long *err = S.get<unsigned long long>(1, "the record table");
     check(cudaMemset(err, 0xff, 8), "cudaMemset");
-    if (n_rec) fq_k_fields<<<grid(n_rec, FQ_THREADS), FQ_THREADS>>>(text, nl, n_nl, n, n_lines, rec_line, n_rec, F.recs, err);
+    if (n_rec) fq_k_fields<<<grid(n_rec, FQ_THREADS), FQ_THREADS>>>(text, nl, n_nl, n, n_lines, rec_line, n_rec, recs, err);
     check(cudaGetLastError(), "fq_k_fields");
-    // the names, gathered into one buffer
-    std::vector<int64_t> spans((size_t)(2 * n_rec)), lo_off((size_t)(2 * n_rec + 1));
-    if (n_rec) check(cudaMemcpy2D(spans.data(), 16, F.recs, sizeof(FastqRec), 16, (size_t)n_rec, cudaMemcpyDeviceToHost), "cudaMemcpy2D");
-    lo_off[(size_t)n_rec] = 0;
+    // the names
+    std::vector<int64_t> spans((size_t)(2 * n_rec)), lo((size_t)n_rec), hi((size_t)n_rec);
+    if (n_rec) check(cudaMemcpy2D(spans.data(), 16, recs, sizeof(FastqRec), 16, (size_t)n_rec, cudaMemcpyDeviceToHost), "cudaMemcpy2D");
     for (int64_t r = 0; r < n_rec; r++) {
-        lo_off[(size_t)r] = spans[(size_t)(2 * r)];
-        lo_off[(size_t)(n_rec + r + 1)] = lo_off[(size_t)(n_rec + r)] + spans[(size_t)(2 * r + 1)] - spans[(size_t)(2 * r)];
+        lo[(size_t)r] = spans[(size_t)(2 * r)];
+        hi[(size_t)r] = spans[(size_t)(2 * r + 1)];
     }
-    const int64_t n_names = lo_off[(size_t)(2 * n_rec)];
-    F.names.resize((size_t)n_names);
-    if (n_names) {
-        const int64_t *idx = upload(S, lo_off.data(), (int64_t)lo_off.size(), "the read names");
-        uint8_t *names = S.get<uint8_t>(n_names, "the read names");
-        bbl_fasta_gather(0, text, idx, idx + n_rec, (int32_t)n_rec, n_names, names);
-        check(cudaGetLastError(), "bbl_fasta_gather");
-        d2h(F.names.data(), names, n_names);
-    }
-    F.name_off.assign(lo_off.begin() + n_rec, lo_off.end());
+    F.name_off = gather_spans(S, 0, text, lo, hi, &F.names, "the read names");
     unsigned long long e = 0;
     d2h(&e, err, 1);
     if (e != ~0ull) {
         const int64_t r = (int64_t)(e >> 1);
-        const std::string name(F.names.data() + F.name_off[(size_t)r], (size_t)(F.name_off[(size_t)r + 1] - F.name_off[(size_t)r]));
+        const std::string name = F.names.substr((size_t)F.name_off[(size_t)r], (size_t)(F.name_off[(size_t)r + 1] - F.name_off[(size_t)r]));
         throw Fail{BB_ERR_ARG, (e & 1) ? "Error: FASTQ record " + std::to_string(r + 1) + " (" + name +
                                              ") is truncated: the file ends before its quality line"
                                        : "Error: FASTQ record " + std::to_string(r + 1) + " has no read name (its header is a lone '@')"};
@@ -178,44 +103,31 @@ extern "C" int bb_device_count(void) {
 
 extern "C" int bb_fastq_parse(int device, const uint8_t *data, int64_t n, int is_gzip, bb_fastq_set **out, int64_t *n_records,
                               int32_t *first_byte) {
-    bbm_set_error("");
-    if (n < 0 || (n > 0 && !data) || !out || !n_records || !first_byte) {
-        bbm_set_error("bb_fastq_parse: invalid argument");
-        return BB_ERR_ARG;
-    }
+    if (n < 0 || (n > 0 && !data) || !out || !n_records || !first_byte) return bad_argument("bb_fastq_parse");
     *out = nullptr;
     *n_records = 0;
     *first_byte = -1;
-    std::unique_ptr<bb_fastq_set> F(new bb_fastq_set());
-    F->device = device;
-    try {
-        check(cudaSetDevice(device), "cudaSetDevice");
-        (void)cudaGetLastError();   // (report this call's launches only)
-        if (is_gzip) {
-            char msg[256];
-            bb_gzip_stats stats{};
-            uint8_t *p = nullptr;
-            const int rc = bbl_gzip_inflate_device(0, data, n, 0, &p, &F->n_text, &stats, msg, sizeof(msg));
-            F->text = p;
-            if (rc) throw Fail{rc, std::string("Error: the FASTQ could not be inflated (") + msg + ")"};
-        } else {
-            F->text = dalloc<uint8_t>(n, "the FASTQ text");
-            F->n_text = n;
-            if (n) check(cudaMemcpy(F->text, data, (size_t)n, cudaMemcpyHostToDevice), "cudaMemcpy");
+    return device_call(device, [&] {
+        std::unique_ptr<bb_fastq_set> F(new bb_fastq_set());
+        F->device = device;
+        Scratch S(BB_ERR_CAPACITY);
+        bb_gzip_stats stats{};
+        try {
+            F->text = text_to_device(S, 0, data, n, is_gzip, &F->n_text, &stats, "the FASTQ text");
+        } catch (const Fail &f) {
+            if (!is_gzip) throw;
+            throw Fail{f.rc, "Error: the FASTQ could not be inflated (" + f.msg + ")"};
         }
         if (F->n_text) {
             uint8_t c = 0;
-            d2h(&c, F->text, 1);
+            d2h(&c, F->text.p, 1);
             *first_byte = c;
         }
         if (*first_byte == '@') parse(*F);
-    } catch (const Fail &f) {
-        bbm_set_error(f.msg.c_str());
-        return f.rc;
-    }
-    *n_records = F->n_rec;
-    *out = F.release();
-    return BB_OK;
+        *n_records = F->n_rec;
+        *out = F.release();
+        return BB_OK;
+    });
 }
 
 extern "C" int bb_fastq_free(bb_fastq_set *F) {
@@ -226,51 +138,45 @@ extern "C" int bb_fastq_free(bb_fastq_set *F) {
 extern "C" int bb_flat_build(bb_fastq_set *F, const bb_aln_view *v, int32_t n_aln, const int64_t *records, const int64_t *contig_at,
                              const int64_t *contig_len, const uint8_t *contigs, int64_t contigs_len, bb_flat_set **out,
                              int64_t *failed, int64_t *slice_len) {
-    bbm_set_error("");
     if (!F || !v || n_aln < 0 || (n_aln && (!records || !contig_at || !contig_len)) || contigs_len < 0 ||
-        (contigs_len && !contigs) || !out || !failed || (n_aln && !F->text)) {
-        bbm_set_error("bb_flat_build: invalid argument");
-        return BB_ERR_ARG;
-    }
+        (contigs_len && !contigs) || !out || !failed || (n_aln && !F->text.p))
+        return bad_argument("bb_flat_build");
     *out = nullptr;
-    std::unique_ptr<bb_flat_set> flat(new bb_flat_set());
-    FqPlan P;
-    const int kind = fq_plan(F->names.data(), F->name_off.data(), F->n_rec, v, n_aln, records, contig_at, contig_len, P, failed);
-    if (kind == 4) {
-        const int32_t id = v->read_id[records[failed[0]]];
-        bbm_set_error(("Error: the CIGAR of read " +
-                       std::string(v->read_names + v->read_name_off[id], (size_t)(v->read_name_off[id + 1] - v->read_name_off[id])) +
-                       " spans more than 2^31 - 1 bases").c_str());
-        failed[0] = -1;
-        failed[1] = 0;
-    }
-    if (kind) return BB_ERR_ARG;
-    const std::vector<FastqAln> &alns = P.alns;
-    const std::vector<uint32_t> &ops = P.ops;
-    const std::vector<int32_t> &p0 = P.p0, &r0 = P.r0;
-    flat->read_off = P.read_off;
-    flat->ref_off = P.ref_off;
-    flat->ops_off = P.ops_off;
-    flat->n = n_aln;
-    const int64_t n_read = flat->read_off.back(), n_ref = flat->ref_off.back(), n_ops = (int64_t)ops.size();
-    try {
-        check(cudaSetDevice(F->device), "cudaSetDevice");
-        (void)cudaGetLastError();
-        Scratch S;
-        flat->read = dalloc<uint8_t>(n_read, "the aligned read slices");
-        flat->qual = dalloc<uint8_t>(n_read, "the aligned quality slices");
-        flat->ref = dalloc<uint8_t>(n_ref, "the aligned reference slices");
-        flat->ops = dalloc<uint32_t>(n_ops, "the CIGAR runs");
-        flat->op_read0 = dalloc<int32_t>(n_ops, "the CIGAR runs");
-        flat->op_ref0 = dalloc<int32_t>(n_ops, "the CIGAR runs");
+    return model_call([&] {
+        FqPlan P;
+        const int kind = fq_plan(F->names.data(), F->name_off.data(), F->n_rec, v, n_aln, records, contig_at, contig_len, P, failed);
+        if (kind == 4) {
+            const int32_t id = v->read_id[records[failed[0]]];
+            failed[0] = -1;
+            failed[1] = 0;
+            throw Fail{BB_ERR_ARG, "Error: the CIGAR of read " +
+                                       std::string(v->read_names + v->read_name_off[id], (size_t)(v->read_name_off[id + 1] - v->read_name_off[id])) +
+                                       " spans more than 2^31 - 1 bases"};
+        }
+        if (kind) return BB_ERR_ARG;
+        const std::vector<FastqAln> &alns = P.alns;
+        std::unique_ptr<bb_flat_set> flat(new bb_flat_set());
+        flat->read_off = P.read_off;
+        flat->ref_off = P.ref_off;
+        flat->ops_off = P.ops_off;
+        flat->n = n_aln;
+        const int64_t n_read = flat->read_off.back(), n_ref = flat->ref_off.back(), n_ops = (int64_t)P.ops.size();
+        use_device(F->device);
+        Scratch S(BB_ERR_CAPACITY);
+        flat->read = S.result((size_t)n_read, "the aligned read slices");
+        flat->qual = S.result((size_t)n_read, "the aligned quality slices");
+        flat->ref = S.result((size_t)n_ref, "the aligned reference slices");
+        flat->ops = S.result((size_t)n_ops * 4, "the CIGAR runs");
+        flat->op_read0 = S.result((size_t)n_ops * 4, "the CIGAR runs");
+        flat->op_ref0 = S.result((size_t)n_ops * 4, "the CIGAR runs");
         if (n_ops) {
-            check(cudaMemcpy(flat->ops, ops.data(), (size_t)n_ops * 4, cudaMemcpyHostToDevice), "cudaMemcpy");
-            check(cudaMemcpy(flat->op_read0, p0.data(), (size_t)n_ops * 4, cudaMemcpyHostToDevice), "cudaMemcpy");
-            check(cudaMemcpy(flat->op_ref0, r0.data(), (size_t)n_ops * 4, cudaMemcpyHostToDevice), "cudaMemcpy");
+            check(cudaMemcpy(flat->ops.p, P.ops.data(), (size_t)n_ops * 4, cudaMemcpyHostToDevice), "cudaMemcpy");
+            check(cudaMemcpy(flat->op_read0.p, P.p0.data(), (size_t)n_ops * 4, cudaMemcpyHostToDevice), "cudaMemcpy");
+            check(cudaMemcpy(flat->op_ref0.p, P.r0.data(), (size_t)n_ops * 4, cudaMemcpyHostToDevice), "cudaMemcpy");
         }
         if (slice_len && n_aln) {   // (the records' spans: the slices' lengths before fq_k_gather pads or truncates them)
             std::vector<FastqRec> recs((size_t)F->n_rec);
-            d2h(recs.data(), F->recs, F->n_rec);
+            d2h(recs.data(), F->recs.p, F->n_rec);
             for (int32_t i = 0; i < n_aln; i++) {
                 const FastqAln &A = alns[(size_t)i];
                 const FastqRec &R = recs[(size_t)A.rec];
@@ -280,17 +186,19 @@ extern "C" int bb_flat_build(bb_fastq_set *F, const bb_aln_view *v, int32_t n_al
                 slice_len[3 * (int64_t)i + 2] = fq_slice(A.contig_len, A.ref_start, A.ref_end, &lo);
             }
         }
-        const FastqAln *d_alns = upload(S, alns.data(), n_aln, "the alignment descriptors");
-        const int64_t *d_read_off = upload(S, flat->read_off.data(), n_aln + 1, "the alignment descriptors");
-        const int64_t *d_ref_off = upload(S, flat->ref_off.data(), n_aln + 1, "the alignment descriptors");
-        const uint8_t *d_contigs = upload(S, contigs, contigs_len, "the reference contigs");
+        const FastqAln *d_alns = S.upload(alns.data(), n_aln, "the alignment descriptors");
+        const int64_t *d_read_off = S.upload(flat->read_off.data(), n_aln + 1, "the alignment descriptors");
+        const int64_t *d_ref_off = S.upload(flat->ref_off.data(), n_aln + 1, "the alignment descriptors");
+        const uint8_t *d_contigs = S.upload(contigs, contigs_len, "the reference contigs");
         uint8_t comp[256];
         bbl_comp_table(comp);
-        const uint8_t *d_comp = upload(S, comp, 256, "the reference contigs");
+        const uint8_t *d_comp = S.upload(comp, 256, "the reference contigs");
         unsigned long long *bad = S.get<unsigned long long>(1, "the alignment descriptors");
         check(cudaMemset(bad, 0xff, 8), "cudaMemset");
-        if (n_aln) fq_k_gather<<<(unsigned)n_aln, FQ_THREADS>>>(F->text, F->recs, d_alns, d_read_off, d_ref_off, d_contigs, d_comp,
-                                                                flat->read, flat->qual, flat->ref, bad);
+        if (n_aln)
+            fq_k_gather<<<(unsigned)n_aln, FQ_THREADS>>>(F->text.as<uint8_t>(), F->recs.as<FastqRec>(), d_alns, d_read_off, d_ref_off,
+                                                        d_contigs, d_comp, flat->read.as<uint8_t>(), flat->qual.as<uint8_t>(),
+                                                        flat->ref.as<uint8_t>(), bad);
         check(cudaGetLastError(), "fq_k_gather");
         unsigned long long b = 0;
         d2h(&b, bad, 1);
@@ -299,24 +207,22 @@ extern "C" int bb_flat_build(bb_fastq_set *F, const bb_aln_view *v, int32_t n_al
             failed[1] = 3;
             return BB_ERR_ARG;
         }
-    } catch (const Fail &f) {
-        bbm_set_error(f.msg.c_str());
-        return f.rc;
-    }
-    F->release();   // (the text and the record table are no longer needed)
-    *out = flat.release();
-    return BB_OK;
+        F->text.release();   // (the text and the record table are no longer needed)
+        F->recs.release();
+        *out = flat.release();
+        return BB_OK;
+    });
 }
 
 extern "C" int bb_flat_view_get(const bb_flat_set *S, bb_flat_view *v) {
     if (!S || !v) return BB_ERR_ARG;
     v->n = S->n;
-    v->read = S->read;
-    v->qual = S->qual;
-    v->ref = S->ref;
-    v->ops = S->ops;
-    v->op_read0 = S->op_read0;
-    v->op_ref0 = S->op_ref0;
+    v->read = S->read.as<uint8_t>();
+    v->qual = S->qual.as<uint8_t>();
+    v->ref = S->ref.as<uint8_t>();
+    v->ops = S->ops.as<uint32_t>();
+    v->op_read0 = S->op_read0.as<int32_t>();
+    v->op_ref0 = S->op_ref0.as<int32_t>();
     v->read_off = S->read_off.data();
     v->ref_off = S->ref_off.data();
     v->ops_off = S->ops_off.data();
@@ -324,25 +230,15 @@ extern "C" int bb_flat_view_get(const bb_flat_set *S, bb_flat_view *v) {
 }
 
 extern "C" int bb_flat_fetch(const bb_flat_set *S, int which, int64_t lo, int64_t count, void *dst) {
-    bbm_set_error("");
-    if (!S || which < 0 || which > 5 || lo < 0 || count < 0 || (count && !dst)) {
-        bbm_set_error("bb_flat_fetch: invalid argument");
-        return BB_ERR_ARG;
-    }
-    const void *src[6] = {S->read, S->qual, S->ref, S->ops, S->op_read0, S->op_ref0};
-    const int64_t size = which < 3 ? 1 : 4;
-    const int64_t total = which < 2 ? S->read_off.back() : which == 2 ? S->ref_off.back() : S->ops_off.back();
-    if (lo + count > total) {
-        bbm_set_error("bb_flat_fetch: range out of bounds");
-        return BB_ERR_ARG;
-    }
-    if (!count) return BB_OK;
-    const cudaError_t e = cudaMemcpy(dst, (const uint8_t *)src[which] + lo * size, (size_t)(count * size), cudaMemcpyDeviceToHost);
-    if (e != cudaSuccess) {
-        bbm_set_error((std::string("bb_flat_fetch: ") + cudaGetErrorString(e)).c_str());
-        return BB_ERR_CUDA;
-    }
-    return BB_OK;
+    if (!S || which < 0 || which > 5 || lo < 0 || count < 0 || (count && !dst)) return bad_argument("bb_flat_fetch");
+    return model_call([&] {
+        const DevBuf *src[6] = {&S->read, &S->qual, &S->ref, &S->ops, &S->op_read0, &S->op_ref0};
+        const int64_t size = which < 3 ? 1 : 4;
+        const int64_t total = which < 2 ? S->read_off.back() : which == 2 ? S->ref_off.back() : S->ops_off.back();
+        if (lo + count > total) throw Fail{BB_ERR_ARG, "bb_flat_fetch: range out of bounds"};
+        if (count) check(cudaMemcpy(dst, src[which]->as<uint8_t>() + lo * size, (size_t)(count * size), cudaMemcpyDeviceToHost), "bb_flat_fetch");
+        return BB_OK;
+    });
 }
 
 extern "C" int bb_flat_free(bb_flat_set *S) {

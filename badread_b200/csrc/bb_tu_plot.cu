@@ -4,69 +4,21 @@
 #include <cuda_runtime.h>
 
 #include <cstdint>
-#include <cstdio>
-#include <string>
 #include <vector>
 
 #include "../../include/badread_b200.h"
 
+#include "bb_call.h"
 #include "bb_plot.cuh"
-
-void bbm_set_error(const char *msg);   // bb_tu_models.cu
-
-namespace {
-
-struct Fail {
-    int rc;
-    std::string msg;
-};
-
-void check(cudaError_t e, const char *what) {
-    if (e != cudaSuccess) throw Fail{BB_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(e)};
-}
-
-struct Scratch {   // what a call allocates, released on every exit path
-    std::vector<void *> p;
-    ~Scratch() { for (void *q : p) cudaFree(q); }
-    template <class X>
-    X *get(int64_t count, const char *what) {
-        const size_t bytes = count * (int64_t)sizeof(X) > 16 ? (size_t)count * sizeof(X) : 16;
-        void *q = nullptr;
-        const cudaError_t e = cudaMalloc(&q, bytes);
-        if (e == cudaErrorMemoryAllocation) {
-            (void)cudaGetLastError();
-            throw Fail{BB_ERR_CAPACITY, std::string("Error: not enough device memory for ") + what + " (" + std::to_string(bytes) +
-                                            " bytes asked for)"};
-        }
-        check(e, "cudaMalloc");
-        p.push_back(q);
-        return (X *)q;
-    }
-    // src[0..count): used in place when it is device memory of `device`, else copied to the device
-    template <class X>
-    const X *input(const X *src, int64_t count, int device, const char *what) {
-        cudaPointerAttributes at{};
-        if (cudaPointerGetAttributes(&at, src) == cudaSuccess && at.type == cudaMemoryTypeDevice && at.device == device) return src;
-        (void)cudaGetLastError();
-        X *d = get<X>(count, what);
-        if (count) check(cudaMemcpy(d, src, (size_t)count * sizeof(X), cudaMemcpyHostToDevice), "cudaMemcpy");
-        return d;
-    }
-};
-
-}  // namespace
 
 extern "C" int bb_window_series(int device, int32_t n_aln, const uint8_t *read, const uint8_t *qual, const uint8_t *ref,
                                 const int64_t *read_off, const int64_t *ref_off, const uint32_t *ops, const int32_t *op_read0,
                                 const int32_t *op_ref0, const int64_t *ops_off, int64_t window, int want_qual, int32_t first_aln,
                                 int32_t n_pass, double *out_identity, double *out_qual, int64_t *n_points) {
-    bbm_set_error("");
     if (n_aln < 0 || first_aln < 0 || n_pass < 0 || (int64_t)first_aln + n_pass > n_aln || window < 1 || !read_off ||
         !ref_off || !ops_off || !n_points || (n_pass && (!read || !ref || !ops || !op_read0 || !op_ref0 || !out_identity)) ||
-        (n_pass && want_qual && (!qual || !out_qual))) {
-        bbm_set_error("bb_window_series: invalid argument");
-        return BB_ERR_ARG;
-    }
+        (n_pass && want_qual && (!qual || !out_qual)))
+        return bad_argument("bb_window_series");
     // pass-local offsets: alignment k = first_aln + k of the pass
     std::vector<int64_t> r_off((size_t)n_pass + 1), f_off((size_t)n_pass + 1), o_off((size_t)n_pass + 1),
         s_off((size_t)n_pass + 1, 0), p_off((size_t)n_pass + 1, 0);
@@ -82,39 +34,34 @@ extern "C" int bb_window_series(int device, int32_t n_aln, const uint8_t *read, 
         }
     }
     *n_points = p_off[(size_t)n_pass];
-    if (n_pass == 0) return BB_OK;
+    if (n_pass == 0) {
+        bbm_set_error("");
+        return BB_OK;
+    }
     const int64_t n_read = r_off.back(), n_ref = f_off.back(), n_ops = o_off.back(), n_pts = p_off.back(), n_sums = s_off.back();
-    try {
-        check(cudaSetDevice(device), "cudaSetDevice");
-        (void)cudaGetLastError();   // (report this call's launch only)
-        Scratch S;
+    return device_call(device, [&] {
+        Scratch S(BB_ERR_CAPACITY);
         const uint8_t *d_read = S.input(read + rb, n_read, device, "the read slices");
         const uint8_t *d_qual = want_qual ? S.input(qual + rb, n_read, device, "the quality slices") : nullptr;
         const uint8_t *d_ref = S.input(ref + fb, n_ref, device, "the reference slices");
         const uint32_t *d_ops = S.input(ops + ob, n_ops, device, "the CIGAR runs");
         const int32_t *d_p0 = S.input(op_read0 + ob, n_ops, device, "the CIGAR runs");
         const int32_t *d_r0 = S.input(op_ref0 + ob, n_ops, device, "the CIGAR runs");
-        int64_t *d_offs = S.get<int64_t>(5 * ((int64_t)n_pass + 1), "the pass offsets");
+        const int64_t n1 = (int64_t)n_pass + 1;
+        int64_t *d_offs = S.get<int64_t>(5 * n1, "the pass offsets");
         const std::vector<int64_t> *offs[5] = {&r_off, &f_off, &o_off, &s_off, &p_off};
         for (int i = 0; i < 5; i++)
-            check(cudaMemcpy(d_offs + i * ((int64_t)n_pass + 1), offs[i]->data(), ((size_t)n_pass + 1) * 8, cudaMemcpyHostToDevice),
-                  "cudaMemcpy");
+            check(cudaMemcpy(d_offs + i * n1, offs[i]->data(), (size_t)n1 * 8, cudaMemcpyHostToDevice), "cudaMemcpy");
         int64_t *d_e = S.get<int64_t>(n_sums, "the error prefix sums");
         int64_t *d_q = want_qual ? S.get<int64_t>(n_sums, "the quality prefix sums") : nullptr;
         double *d_id = S.get<double>(n_pts, "the identity series");
         double *d_mq = want_qual ? S.get<double>(n_pts, "the qscore series") : nullptr;
-        const int64_t n1 = (int64_t)n_pass + 1;
         ws_k_series<<<(unsigned)n_pass, WS_THREADS>>>(d_read, d_qual, d_ref, d_offs, d_offs + n1, d_ops, d_p0, d_r0, d_offs + 2 * n1,
                                                       window, WS_ITEMS, d_offs + 3 * n1, d_offs + 4 * n1, d_e, d_q, d_id, d_mq);
         check(cudaGetLastError(), "ws_k_series");
-        if (n_pts) {
-            check(cudaMemcpy(out_identity, d_id, (size_t)n_pts * 8, cudaMemcpyDeviceToHost), "cudaMemcpy");
-            if (want_qual) check(cudaMemcpy(out_qual, d_mq, (size_t)n_pts * 8, cudaMemcpyDeviceToHost), "cudaMemcpy");
-        }
+        d2h(out_identity, d_id, n_pts);
+        if (want_qual) d2h(out_qual, d_mq, n_pts);
         check(cudaDeviceSynchronize(), "ws_k_series");
-    } catch (const Fail &f) {
-        bbm_set_error(f.msg.c_str());
-        return f.rc;
-    }
-    return BB_OK;
+        return BB_OK;
+    });
 }
