@@ -1,12 +1,13 @@
-// bb_call.h — how the loader and model-builder entry points own device memory and report failures, and the host helpers
-// of the input paths that more than one unit calls.  The entry points that take a device instead of a context report
-// through bb_model_error(), a message per host thread; a helper that fails throws Fail, and one wrapper per entry point
-// turns it into the return code and the message.  The first half is plain C++, for the units g++ compiles without the
-// CUDA headers (bb_bam.cpp); the rest needs cuda_runtime.h.
+// bb_call.h — how the entry points own device memory and report failures, and the host helpers of the input paths that
+// more than one unit calls.  A helper that fails throws Fail, and one wrapper per entry point turns it into the return
+// code and the message: bb_last_error() of the context for the context entry points (context_call), bb_model_error(), a
+// message per host thread, for the loaders and model builders, which take a device instead (model_call).  The first
+// half is plain C++, for the units g++ compiles without the CUDA headers (bb_bam.cpp); the rest needs cuda_runtime.h.
 #pragma once
 #include <algorithm>
 #include <cstdint>
 #include <string>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -61,15 +62,32 @@ int device_call(int device, F &&body) {
     });
 }
 
-// The same conversion for a context's entry points, whose message bb_last_error() reports
-template <class F>
-int context_call(std::string &err, F &&body) {
+// Runs a context entry point's body(), which returns its code or nothing (BB_OK).  A null context is refused with
+// BB_ERR_ARG and no message; a Fail becomes the code and the context's message (bb_last_error), which a success leaves
+// as it was.
+template <class Ctx, class F>
+int context_call(Ctx *ctx, F &&body) {
+    if (!ctx) return BB_ERR_ARG;
     try {
-        return body();
+        if constexpr (std::is_void_v<decltype(body())>) {
+            body();
+            return BB_OK;
+        } else {
+            return body();
+        }
     } catch (const Fail &f) {
-        err = f.msg;
+        ctx->err = f.msg;
         return f.rc;
     }
+}
+
+// context_call for an entry point that works on the context's device: body() runs with it current (use_device)
+template <class Ctx, class F>
+int context_device_call(Ctx *ctx, F &&body) {
+    return context_call(ctx, [&] {
+        use_device(ctx->device);
+        return body();
+    });
 }
 
 struct DevBuf {   // a device allocation, freed with its owner
@@ -88,14 +106,15 @@ struct DevBuf {   // a device allocation, freed with its owner
         return *this;
     }
     ~DevBuf() { release(); }
-    // grow-only: at least `bytes`, with slack for the next call
-    cudaError_t ensure(size_t bytes) {
-        if (bytes <= cap) return cudaSuccess;
+    // grow-only: at least `bytes`, with slack for the next call; a failure throws BB_ERR_CUDA "<what>: <error>"
+    void ensure(size_t bytes, const char *what) {
+        if (bytes <= cap) return;
         release();
         const size_t want = bytes + bytes / 8 + 256;
         const cudaError_t e = cudaMalloc(&p, want);
-        if (e == cudaSuccess) cap = want;
-        return e;
+        if (e != cudaSuccess) (void)cudaGetLastError();   // (an out-of-memory, say, is not for a later launch to report)
+        check(e, what);
+        cap = want;
     }
     // exactly `bytes` (at least 1), for buffers the size of their contents
     cudaError_t alloc(size_t bytes) {
